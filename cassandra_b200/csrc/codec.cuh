@@ -283,7 +283,8 @@ __global__ void k_digest_final(const DevTables* __restrict__ T, const uint64_t* 
 __global__ void __launch_bounds__(64) k_decompress_chunks(const DevTables* __restrict__ T, int comp,
         const uint8_t* __restrict__ data, uint64_t data_len, const uint64_t* __restrict__ offs, uint64_t nchunks,
         int chunk_len, int max_clen, uint64_t data_length, uint8_t* out, int verify, ChunkErr* __restrict__ err,
-        uint64_t chunk0, uint64_t chunk_end, int tag) {        // this launch covers chunks [chunk0, chunk_end) of the file; tag = input number for error reports
+        uint64_t chunk0, uint64_t chunk_end, int tag,         // this launch covers chunks [chunk0, chunk_end) of the file; tag = input number for error reports
+        const uint8_t* __restrict__ tail, uint64_t tail_off) {  // (k1_src)
     const int lane = threadIdx.x & 31;
     const uint64_t chunk = chunk0 + (uint64_t)blockIdx.x * 2 + (threadIdx.x >> 5);
     if (chunk >= chunk_end || chunk >= nchunks) return;
@@ -296,7 +297,7 @@ __global__ void __launch_bounds__(64) k_decompress_chunks(const DevTables* __res
     }
     const int clen = (int)(next - off - 4);
     const int ulen = (int)min((uint64_t)chunk_len, data_length - ustart);
-    const uint8_t* src = data + off;
+    const uint8_t* src = k1_src(data, tail, tail_off, off);
     if (verify) {
         uint32_t crc = warp_crc32(T, T->crc_adv128, src, clen, lane);
         uint32_t stored = ((uint32_t)src[clen] << 24) | ((uint32_t)src[clen + 1] << 16) | ((uint32_t)src[clen + 2] << 8) | src[clen + 3];
@@ -327,7 +328,8 @@ __global__ void __launch_bounds__(64) k_decompress_chunks(const DevTables* __res
 // sources are read with two aligned 64-bit loads + a funnel shift. CRC32: slice-by-4 with the tables in shared memory.
 __device__ __forceinline__ void decompress_chunk_thread(const uint32_t (*s_crc)[256], int comp,
         const uint8_t* __restrict__ data, uint64_t data_len, const uint64_t* __restrict__ offs, uint64_t nchunks,
-        int chunk_len, int max_clen, uint64_t data_length, uint8_t* out, int verify, ChunkErr* __restrict__ err, uint64_t chunk, int tag) {
+        int chunk_len, int max_clen, uint64_t data_length, uint8_t* out, int verify, ChunkErr* __restrict__ err, uint64_t chunk, int tag,
+        const uint8_t* __restrict__ tail, uint64_t tail_off) {
     const uint64_t off = offs[chunk];
     const uint64_t next = (chunk + 1 < nchunks) ? offs[chunk + 1] : data_len;
     const uint64_t ustart = chunk * (uint64_t)chunk_len;
@@ -335,7 +337,7 @@ __device__ __forceinline__ void decompress_chunk_thread(const uint32_t (*s_crc)[
     if (off + 4 > next || next > data_len || ustart >= data_length || next - off - 4 > (uint64_t)(chunk_max_compressed(comp, chunk_len) + chunk_len)) { report_chunk_err(err, ctag, 2); return; }
     const int clen = (int)(next - off - 4);
     const int ulen = (int)min((uint64_t)chunk_len, data_length - ustart);
-    const uint8_t* src = data + off;
+    const uint8_t* src = k1_src(data, tail, tail_off, off);
     if (verify) {
         uint32_t crc = 0xFFFFFFFFu; int i = 0;
         // a thread's chunk is its private stream: fetching it 8 bytes at a time asks for every 32-byte sector four times, with a few thousand
@@ -380,32 +382,42 @@ __device__ __forceinline__ void decompress_chunk_thread(const uint32_t (*s_crc)[
     if (got != ulen) report_chunk_err(err, ctag, 2);
 }
 
-__global__ void __launch_bounds__(128) k_decompress_chunks_thr(const DevTables* __restrict__ T, int comp,
+// threads per block of the two kernels below, their static shared memory (the CRC tables), and the L2 bytes each chunk in flight is
+// given (engine.cu: k1_plan). 768: 4 blocks of 128 per SM on an H100 (50 MiB L2, 132 SMs) — the fastest point of the curve measured
+// on configs[1] (DESIGN §7: 2 blocks 71 ms, 3: 60, 4: 58, 6: 75; all 12 the registers allow: 138).
+enum { K1_THREADS = 128, K1_STATIC_SMEM = 4 * 256 * 4 };
+constexpr uint64_t K1_L2_BYTES_PER_CHAIN = 768;
+
+__global__ void __launch_bounds__(K1_THREADS) k_decompress_chunks_thr(const DevTables* __restrict__ T, int comp,
         const uint8_t* __restrict__ data, uint64_t data_len, const uint64_t* __restrict__ offs, uint64_t nchunks,
         int chunk_len, int max_clen, uint64_t data_length, uint8_t* out, int verify, ChunkErr* __restrict__ err,
-        uint64_t chunk0, uint64_t chunk_end, int tag) {
+        uint64_t chunk0, uint64_t chunk_end, int tag, const uint8_t* __restrict__ tail, uint64_t tail_off) {
     __shared__ uint32_t s_crc[4][256];
     for (int i = threadIdx.x; i < 1024; i += blockDim.x) s_crc[i >> 8][i & 255] = T->crc_t[i >> 8][i & 255];
     __syncthreads();
-    const uint64_t chunk = chunk0 + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (chunk >= chunk_end || chunk >= nchunks) return;
-    decompress_chunk_thread(s_crc, comp, data, data_len, offs, nchunks, chunk_len, max_clen, data_length, out, verify, err, chunk, tag);
+    if (chunk_end > nchunks) chunk_end = nchunks;
+    for (uint64_t chunk = chunk0 + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; chunk < chunk_end; chunk += (uint64_t)gridDim.x * blockDim.x)
+        decompress_chunk_thread(s_crc, comp, data, data_len, offs, nchunks, chunk_len, max_clen, data_length, out, verify, err, chunk, tag, tail, tail_off);
 }
 
-// the same over chunk ranges of several inputs in ONE launch: thread-per-chunk only pays off with >= ~10^5 chunks in flight
-__global__ void __launch_bounds__(128) k_decompress_multi_thr(const DevTables* __restrict__ T, const K1Seg* __restrict__ segs, int nseg, uint64_t total,
-                                                              int verify, ChunkErr* __restrict__ err) {
+// the same over chunk ranges of several inputs in ONE launch. Both thread kernels loop over their chunks in launch order; the grid is
+// sized by k1_grid (engine.cu) so that the chunks in flight keep their working set in the caches. Here a thread that finishes takes the
+// next chunk from a counter (`next`, zeroed by the launch): no thread waits behind a slow chunk's neighbours.
+__global__ void __launch_bounds__(K1_THREADS) k_decompress_multi_thr(const DevTables* __restrict__ T, const K1Seg* __restrict__ segs, int nseg, uint64_t total,
+                                                              int verify, ChunkErr* __restrict__ err, unsigned long long* __restrict__ next) {
     __shared__ uint32_t s_crc[4][256];
     for (int i = threadIdx.x; i < 1024; i += blockDim.x) s_crc[i >> 8][i & 255] = T->crc_t[i >> 8][i & 255];
     __syncthreads();
-    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= total) return;
-    int lo = 0, hi = nseg - 1;
-    while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (segs[mid].first <= t) lo = mid; else hi = mid - 1; }
-    const K1Seg g = segs[lo];
-    const uint64_t chunk = g.chunk0 + (t - g.first);
-    if (chunk >= g.nchunks) return;
-    decompress_chunk_thread(s_crc, COMP_LZ4, g.data, g.data_len, g.offs, g.nchunks, g.chunk_len, g.max_clen, g.data_length, g.out, verify, err, chunk, g.tag);
+    const uint64_t G = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t = G + atomicAdd(next, 1ull)) {
+        int lo = 0, hi = nseg - 1;
+        while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (segs[mid].first <= t) lo = mid; else hi = mid - 1; }
+        const K1Seg g = segs[lo];
+        const uint64_t chunk = g.chunk0 + (t - g.first);
+        if (chunk >= g.nchunks) continue;
+        decompress_chunk_thread(s_crc, COMP_LZ4, g.data, g.data_len, g.offs, g.nchunks, g.chunk_len, g.max_clen, g.data_length, g.out, verify, err, chunk, g.tag,
+                                g.tail, g.tail_off);
+    }
 }
 
 // ---- K1 in two passes (lz4_batch.cuh): walk (thread per chunk: validate, record the sequence starts) then copy (warp per chunk, 32 sequences
@@ -426,7 +438,7 @@ __device__ __forceinline__ uint32_t k1_locate(const K1Seg* __restrict__ segs, in
     if (off + 4 > next || next > g.data_len || ustart >= g.data_length || next - off - 4 > (uint64_t)(chunk_max_compressed(COMP_LZ4, g.chunk_len) + g.chunk_len) ||
         off < off0 || next - off0 > g.rec_span) return K1_BAD_OFFS;
     k.clen = (int)(next - off - 4); k.ulen = (int)min((uint64_t)g.chunk_len, g.data_length - ustart);
-    k.src = g.data + off; k.dst = g.out + ustart;
+    k.src = k1_src(g.data, g.tail, g.tail_off, off); k.dst = g.out + ustart;
     k.slot = g.rec0 + (off - off0) / 3 + 2 * (chunk - g.chunk0);
     return k.clen >= g.max_clen ? K1_RAW : 0u;
 }

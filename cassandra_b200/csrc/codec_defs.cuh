@@ -1,6 +1,7 @@
 // codec_defs.cuh — chunk codec constants shared by the codec kernels (codec.cuh) and the compaction driver (compact.cu).
 #pragma once
 #include "common.cuh"
+#include "k1_tail.cuh"
 
 namespace b200c {
 
@@ -26,6 +27,7 @@ __device__ __forceinline__ void report_chunk_err(ChunkErr* e, uint64_t chunk, in
 // one input's chunk range [chunk0, chunk0 + count) in a multi-input K1 launch; first = threads of the launch before this segment
 struct K1Seg { const uint8_t* data; uint64_t data_len; const uint64_t* offs; uint64_t nchunks; uint64_t data_length; uint8_t* out;
                uint64_t chunk0, count, first; int chunk_len, max_clen, tag, _pad;
-               uint64_t rec0, rec_span; };      // two-pass LZ4 (lz4_batch.cuh): first record slot of this segment, compressed bytes its slots were sized for
+               uint64_t rec0, rec_span;         // two-pass LZ4 (lz4_batch.cuh): first record slot of this segment, compressed bytes its slots were sized for
+               const uint8_t* tail; uint64_t tail_off; };     // staged copy of the file's bytes from tail_off on (k1_src)
 
 } // namespace b200c

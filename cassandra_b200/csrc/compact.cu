@@ -35,7 +35,8 @@ int compress_slots_device(b200c_ctx* c, int comp, const uint8_t* d_in, uint64_t 
 int pack_digest_device(b200c_ctx* c, const uint8_t* slots, int stride, const uint32_t* file_len, const uint32_t* seg_raw, uint64_t nchunks,
                        uint8_t* d_out, uint64_t out_cap, uint64_t* d_offs, uint64_t* out_len, uint32_t* digest, int ws_base);
 int decompress_stream_device(b200c_ctx* c, int comp, const uint8_t* d_data, uint64_t data_len, const uint64_t* d_offs, uint64_t nchunks,
-                             int chunk_len, int max_clen, uint64_t data_length, uint8_t* d_out, int verify, ChunkErr* d_err, uint64_t chunk0, uint64_t count, int tag);
+                             int chunk_len, int max_clen, uint64_t data_length, uint8_t* d_out, int verify, ChunkErr* d_err, uint64_t chunk0, uint64_t count, int tag,
+                             const uint8_t* tail, uint64_t tail_off);
 int decompress_multi_device(b200c_ctx* c, K1Seg* segs, int nseg, int verify, ChunkErr* d_err, int ws_slot);
 
 enum { IB = 256 };                       // Index.db speculation block
@@ -50,10 +51,10 @@ enum { MAX_RANGES = 16, EV_RANGE = 200, EV_INDEX = 220, EV_K5 = 230 };      // t
 
 enum { WS_U = 16, WS_CD, WS_CO, WS_IDX, WS_PARAMS, WS_BBASE, WS_ISTART, WS_ICNT, WS_IEND, WS_IHIT, WS_IBAD, WS_ISCAN,
        WS_TOK, WS_KP, WS_KLEN, WS_UPOS, WS_PBASE, WS_RANGE, WS_BSTART, WS_CONTRIB, WS_HEAD, WS_OPIDX, WS_OPFIRST,
-       WS_LIST, WS_CURSOR, WS_STMUNF, WS_STROWS, WS_OVF, WS_BOUND, WS_BPOS, WS_SCRATCH, WS_DSIZE, WS_IPAY, WS_NBLK, WS_IHEAD, WS_DPOS, WS_ISIZE, WS_IPOS, WS_UOUT, WS_IOUT, WS_DOUT, WS_OOFFS, WS_STATS, WS_ERR2, WS_LCS0 = 82, WS_LCS1, WS_LCS2, WS_LCS3, WS_LCS4, WS_ICAP, WS_IOFF, WS_ISCR, WS_PLAN, WS_UOUT2, WS_SUMM, WS_PURGE, WS_K1SEG, WS_INSZ, WS_BIG, WS_INPOS, WS_TMARK, WS_TSCAN, WS_TSTART, WS_META_SG, WS_META_TD, WS_META_BLOOM, WS_META_KEYS, WS_META_SUMENT, WS_META_SUMOFF, WS_META_FLAG, WS_META_WRANK, WS_META_SAMPLE, WS_META_ESIZE, WS_META_EPOS, WS_CCOUNT, WS_SLICE, WS_META_TDD,
+       WS_LIST, WS_CURSOR, WS_STMUNF, WS_STROWS, WS_OVF, WS_BOUND, WS_BPOS, WS_SCRATCH, WS_DSIZE, WS_IPAY, WS_NBLK, WS_IHEAD, WS_DPOS, WS_ISIZE, WS_IPOS, WS_UOUT, WS_IOUT, WS_DOUT, WS_OOFFS, WS_STATS, WS_ERR2, WS_LCS0 = 82, WS_LCS1, WS_LCS2, WS_LCS3, WS_LCS4, WS_ICAP, WS_IOFF, WS_ISCR, WS_PLAN, WS_UOUT2, WS_SUMM, WS_PURGE, WS_K1SEG, WS_INSZ, WS_BIG, WS_INPOS, WS_TMARK, WS_TSCAN, WS_TSTART, WS_META_SG, WS_META_TD, WS_META_BLOOM, WS_META_KEYS, WS_META_SUMENT, WS_META_SUMOFF, WS_META_FLAG, WS_META_WRANK, WS_META_SAMPLE, WS_META_ESIZE, WS_META_EPOS, WS_CCOUNT, WS_SLICE, WS_META_TDD, WS_K1TAIL,
        WS_SCANA = 60, WS_CODEC = 70 };
 
-static_assert(WS_ERR2 < WS_SCANA && WS_SCANA + 6 <= WS_CODEC && WS_CODEC + 12 <= WS_LCS0 && WS_META_TDD < WS_SLOTS, "workspace slot map");
+static_assert(WS_ERR2 < WS_SCANA && WS_SCANA + 6 <= WS_CODEC && WS_CODEC + 12 <= WS_LCS0 && WS_K1TAIL < WS_SLOTS, "workspace slot map");
 struct DevErr { unsigned long long code; };       // min over (kind << 56 | input << 48 | offset); ~0 = none
 
 __device__ __forceinline__ void report_err(DevErr* e, int kind, int input, uint64_t off) {
@@ -1106,8 +1107,25 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
     const int nr = (int)T.size() - 1;
     uint8_t *U, *CD, *IDX; uint64_t* CO; CParams* dP; uint64_t* d_bbase; DevErr* d_err; ChunkErr* d_cerr; RunStats* d_stats; unsigned long long* d_hist;
     B200C_TRY(ws_typed(c, WS_U, uo + 64, &U));
-    B200C_TRY(ws_typed(c, WS_CD, co + 64, &CD));
-    B200C_TRY(ws_typed(c, WS_CO, oo + 1, &CO));
+    // K1's view of input i. Host inputs are staged in CD / CO. Device-resident inputs are read where the caller keeps them: no copy,
+    // no second image of the compressed inputs in device memory; only the file's tail is staged for the decoders' word reads (k1_src).
+    std::vector<const uint8_t*> k1_data(K), k1_tail(K, nullptr); std::vector<const uint64_t*> k1_offs(K); std::vector<uint64_t> k1_tail_off(K, ~0ull);
+    if (dev) {
+        std::vector<uint64_t> tb(K + 1, 0);
+        for (int i = 0; i < K; i++) tb[i + 1] = tb[i] + ((std::min(m->inputs[i].data_len, k1_tail_window(chunk_max_compressed(m->inputs[i].compressor, m->inputs[i].chunk_len), m->inputs[i].chunk_len)) + 64 + 15) & ~15ull);
+        uint8_t* TAIL; B200C_TRY(ws_typed(c, WS_K1TAIL, tb[K] + 64, &TAIL));
+        CD = nullptr; CO = nullptr;
+        for (int i = 0; i < K; i++) {
+            const b200c_input& in = m->inputs[i];
+            const uint64_t win = std::min(in.data_len, k1_tail_window(chunk_max_compressed(in.compressor, in.chunk_len), in.chunk_len));
+            k1_data[i] = in.data; k1_offs[i] = in.chunk_offsets; k1_tail[i] = TAIL + tb[i]; k1_tail_off[i] = in.data_len - win;
+            if (win) B200C_CUDA_TRY(c, cudaMemcpyAsync(TAIL + tb[i], in.data + (in.data_len - win), win, cudaMemcpyDeviceToDevice, c->stream));
+        }
+    } else {
+        B200C_TRY(ws_typed(c, WS_CD, co + 64, &CD));
+        B200C_TRY(ws_typed(c, WS_CO, oo + 1, &CO));
+        for (int i = 0; i < K; i++) { k1_data[i] = CD + cbase[i]; k1_offs[i] = CO + obase[i]; }
+    }
     B200C_TRY(ws_typed(c, WS_IDX, io + 64, &IDX));
     // Summary.db positions on the device: one run per piece and input (file offsets; K2 subtracts the slice start — no kernel rides on the copy stream)
     std::vector<std::vector<uint64_t>> psb(nr, std::vector<uint64_t>(K + 1, 0));
@@ -1167,9 +1185,9 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
     }
     if (!co_host.empty()) B200C_CUDA_TRY(c, cudaStreamSynchronize(cs));
     auto chunk_off = [&](int i, uint64_t ch) -> uint64_t { const b200c_input& in = m->inputs[i]; return ch >= in.nchunks ? in.data_len : (co_host.empty() ? in.chunk_offsets[ch] : co_host[i][ch]); };
-    auto copy_chunks = [&](int i, uint64_t a, uint64_t b) -> int {      // compressed bytes of chunks [a, b) of input i -> CD
+    auto copy_chunks = [&](int i, uint64_t a, uint64_t b) -> int {      // compressed bytes of chunks [a, b) of input i -> CD (host inputs)
         const b200c_input& in = m->inputs[i];
-        if (a >= b) return B200C_OK;
+        if (a >= b || dev) return B200C_OK;
         uint64_t lo = chunk_off(i, a), hi = chunk_off(i, b);
         if (lo > hi || hi > in.data_len) { c->err = "chunk offsets of input " + std::to_string(i) + " are not increasing"; res->corruption.input = i; res->corruption.kind = 2; res->corruption.chunk = a; res->corruption.offset = 0; return B200C_ECORRUPT; }
         if (hi > lo) B200C_CUDA_TRY(c, cudaMemcpyAsync(CD + cbase[i] + lo, in.data + lo, hi - lo, kind, cs));
@@ -1194,8 +1212,8 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
     };
     for (int i = 0; i < K; i++) {
         const b200c_input& in = m->inputs[i];
-        if (!deferred && in.data_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(CD + cbase[i], in.data, in.data_len, kind, cs));
-        if (in.nchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(CO + obase[i], in.chunk_offsets, in.nchunks * 8, kind, cs));
+        if (!dev && !deferred && in.data_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(CD + cbase[i], in.data, in.data_len, kind, cs));
+        if (!dev && in.nchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(CO + obase[i], in.chunk_offsets, in.nchunks * 8, kind, cs));
         if (!istream) {
             if (isl[i].hi > isl[i].lo) B200C_CUDA_TRY(c, cudaMemcpyAsync(IDX + ibase[i], in.index + isl[i].lo, isl[i].hi - isl[i].lo, kind, cs));
             if (isl[i].s_count) {
@@ -1254,8 +1272,8 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
     auto k1 = [&](int i, uint64_t a, uint64_t b) -> int {           // chunks [a, b) of input i
         const b200c_input& in = m->inputs[i];
         if (a >= b) return B200C_OK;
-        return decompress_stream_device(c, in.compressor, CD + cbase[i], in.data_len, CO + obase[i], in.nchunks, in.chunk_len,
-                                        in.max_compressed_len, in.data_length, U + ubase[i], 1, d_cerr, a, b - a, i);
+        return decompress_stream_device(c, in.compressor, k1_data[i], in.data_len, k1_offs[i], in.nchunks, in.chunk_len,
+                                        in.max_compressed_len, in.data_length, U + ubase[i], 1, d_cerr, a, b - a, i, k1_tail[i], k1_tail_off[i]);
     };
     // several inputs' chunk ranges in one thread-per-chunk launch when there are enough of them (B200C_K1_BATCH=0 switches it off)
     const int k1_batch_env = []() { const char* e = getenv("B200C_K1_BATCH"); return e ? atoi(e) : (B200C_K1_BATCH_DEFAULT ? 1 : 0); }();     // 2: batch even tiny launches (tests)
@@ -1267,7 +1285,8 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
             const b200c_input& in = m->inputs[i];
             if (from[i] >= to[i] || in.compressor != COMP_LZ4 || (in.chunk_len & 7)) continue;
             K1Seg g; memset(&g, 0, sizeof(g));
-            g.data = CD + cbase[i]; g.data_len = in.data_len; g.offs = CO + obase[i]; g.nchunks = in.nchunks; g.data_length = in.data_length; g.out = U + ubase[i];
+            g.data = k1_data[i]; g.data_len = in.data_len; g.offs = k1_offs[i]; g.nchunks = in.nchunks; g.data_length = in.data_length; g.out = U + ubase[i];
+            g.tail = k1_tail[i]; g.tail_off = k1_tail_off[i];
             g.chunk0 = from[i]; g.count = to[i] - from[i]; g.chunk_len = in.chunk_len; g.max_clen = in.max_compressed_len; g.tag = i;
             if (!dev || !co_host.empty()) { const uint64_t a = chunk_off(i, from[i]), b = chunk_off(i, to[i]); g.rec_span = b > a ? b - a : 0; }      // (0 / unknown: the whole file)
             segs.push_back(g); total += g.count;
@@ -1281,9 +1300,12 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         }
         return B200C_OK;
     };
-    for (int i = 0; i < K; i++) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_in[i], 0));      // chunk offsets (and, unless the pieces bring their own, Index.db / Data.db) are there
+    // K1 waits for what it reads: host inputs' chunk offsets and (unless the pieces bring their own) Data.db. Device-resident inputs are
+    // read in place; their Index.db / Summary.db staging runs under K1 and K2 waits for it.
+    auto wait_inputs = [&]() -> int { for (int i = 0; i < K; i++) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_in[i], 0)); return B200C_OK; };
+    if (!dev) B200C_TRY(wait_inputs());
     if (!deferred) {
-        if (dev && k1_batching) {          // device-resident inputs: the staging copies are device-to-device, decode in one launch
+        if (dev && k1_batching) {          // device-resident inputs: decode in one launch
             std::vector<uint64_t> z(K, 0), e(K);
             for (int i = 0; i < K; i++) e[i] = m->inputs[i].nchunks;
             B200C_TRY(k1_many(z, e));
@@ -1440,6 +1462,7 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         return B200C_OK;
     };
     mark(1);
+    if (dev) B200C_TRY(wait_inputs());
     if (!istream) B200C_TRY(k2_run(isl, psb[0], m->token_lo, m->token_hi));
 
     // ---- token ranges: T[0] < T[1] < ... < T[nr]; piece r merges the partitions with token in (T[r], T[r+1]]. Several pieces: planned on the

@@ -213,21 +213,47 @@ int out_stream_finish(OutStream& o, uint64_t* out_len, uint32_t* digest, uint64_
     return B200C_OK;
 }
 
-// chunks [chunk0, chunk0 + count) of the file (count = ~0: through the last chunk)
+// Geometry of the thread-per-chunk K1 kernels. Every chunk in flight is a private chain of dependent loads that touches its compressed
+// bytes twice (CRC, decode), its output sectors once per 8-byte store and its own recent output for every match: once the chains in
+// flight need more than the caches hold, those bytes come from DRAM again and every dependent load waits longer. So the kernels loop
+// over their chunks and a launch keeps L2 size / K1_L2_BYTES_PER_CHAIN of them in flight, in whole blocks per SM (k1_plan, at
+// context creation). A grid of that size alone would let the block scheduler stack blocks on some SMs, so each block also asks for
+// (unused) dynamic shared memory: exactly that many blocks fill the smallest shared-memory carveout that holds them, and the rest of
+// the SM's 256 KB stays L1 for the chains (a carveout sized for the maximum shared memory leaves ~28 KB of L1: K1 then took 80 ms
+// instead of 58 on configs[1], DESIGN §7).
+static void k1_plan(b200c_ctx* c) {
+    static const int carveout_kb[] = {0, 8, 16, 32, 64, 100, 132, 164, 196, 228};      // the shared-memory capacities an sm_90 SM supports
+    const int per_sm = (int)std::max<uint64_t>(1, (uint64_t)c->l2_bytes / K1_L2_BYTES_PER_CHAIN / K1_THREADS / (uint64_t)c->nsm);
+    const int block = c->smem_reserved_per_block + K1_STATIC_SMEM;
+    int carve = c->smem_per_sm;
+    for (int kb : carveout_kb) if (kb * 1024 >= per_sm * block) { carve = std::min(kb * 1024, c->smem_per_sm); break; }
+    c->k1_blocks_per_sm = per_sm;
+    c->k1_smem = (size_t)std::max(0, (carve / per_sm - block) & ~127);
+    for (const void* k : {(const void*)k_decompress_multi_thr, (const void*)k_decompress_chunks_thr}) {
+        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->k1_smem);
+        cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, 100 * carve / c->smem_per_sm);
+    }
+}
+static unsigned k1_grid(const b200c_ctx* c, uint64_t nthreads) {
+    return (unsigned)std::min<uint64_t>((uint64_t)c->k1_blocks_per_sm * (uint64_t)c->nsm, (nthreads + K1_THREADS - 1) / K1_THREADS);
+}
+
+// chunks [chunk0, chunk0 + count) of the file (count = ~0: through the last chunk); chunks from file offset tail_off on are read
+// from `tail` (k1_src; tail_off = ~0: none)
 int decompress_stream_device(b200c_ctx* c, int comp, const uint8_t* d_data, uint64_t data_len, const uint64_t* d_offs, uint64_t nchunks,
                              int chunk_len, int max_clen, uint64_t data_length, uint8_t* d_out, int verify, ChunkErr* d_err,
-                             uint64_t chunk0, uint64_t count, int tag) {
+                             uint64_t chunk0, uint64_t count, int tag, const uint8_t* tail, uint64_t tail_off) {
     if (chunk0 >= nchunks || count == 0) return B200C_OK;
     const uint64_t end = count > nchunks - chunk0 ? nchunks : chunk0 + count;
     static const int k1_mode = []() { const char* e = getenv("B200C_K1"); return e ? atoi(e) : 1; }();      // 0: warp per chunk, 1: thread per chunk (LZ4)
     // thread per chunk needs tens of thousands of chunks in flight to beat the warp kernel; small launches (token-range pieces of one
     // input) keep the warp mapping unless compact.cu has batched them (decompress_multi_device)
     if (k1_mode == 1 && comp == COMP_LZ4 && (chunk_len & 7) == 0 && ((uintptr_t)d_out & 7) == 0 && end - chunk0 >= 32768)
-        B200C_LAUNCH(c, k_decompress_chunks_thr, (unsigned)((end - chunk0 + 127) / 128), 128, 0, c->d_tables, comp, d_data, data_len, d_offs, nchunks,
-                     chunk_len, max_clen, data_length, d_out, verify, d_err, chunk0, end, tag);
+        B200C_LAUNCH(c, k_decompress_chunks_thr, k1_grid(c, end - chunk0), K1_THREADS, c->k1_smem, c->d_tables, comp, d_data, data_len, d_offs, nchunks,
+                     chunk_len, max_clen, data_length, d_out, verify, d_err, chunk0, end, tag, tail, tail_off);
     else
         B200C_LAUNCH(c, k_decompress_chunks, (unsigned)((end - chunk0 + 1) / 2), 64, 0, c->d_tables, comp, d_data, data_len, d_offs, nchunks,
-                     chunk_len, max_clen, data_length, d_out, verify, d_err, chunk0, end, tag);
+                     chunk_len, max_clen, data_length, d_out, verify, d_err, chunk0, end, tag, tail, tail_off);
     return B200C_OK;
 }
 
@@ -244,7 +270,7 @@ int decompress_multi_device(b200c_ctx* c, K1Seg* segs, int nseg, int verify, Chu
         if (!segs[i].rec_span || segs[i].rec_span > segs[i].data_len) segs[i].rec_span = segs[i].data_len;
         segs[i].rec0 = rec_total; rec_total += segs[i].rec_span / 3 + 2 * segs[i].count + 8;
     }
-    K1Seg* d; B200C_TRY(ws_typed(c, ws_slot, (size_t)nseg, &d));
+    K1Seg* d; B200C_TRY(ws_typed(c, ws_slot, (size_t)nseg + 1, &d));
     B200C_CUDA_TRY(c, cudaMemcpyAsync(d, segs, sizeof(K1Seg) * nseg, cudaMemcpyHostToDevice, c->stream));
     if (k1_mode == 2) {
         uint16_t* rec; uint32_t* nseq;
@@ -258,11 +284,9 @@ int decompress_multi_device(b200c_ctx* c, K1Seg* segs, int nseg, int verify, Chu
         B200C_LAUNCH(c, k_lz4_copy_multi, (unsigned)((total + K1C_WARPS - 1) / K1C_WARPS), 32 * K1C_WARPS, pad, c->d_tables, (const K1Seg*)d, nseg, total, (const uint16_t*)rec, (const uint32_t*)nseq, verify, d_err);
         return B200C_OK;
     }
-    // B200C_K1_PAD=bytes of unused dynamic shared memory per block: caps the blocks resident per SM (A/B: fewer private streams in flight =
-    // a smaller L2 working set for a kernel whose DRAM traffic is several times its algorithmic bytes)
-    const int k1_pad = []() { const char* e = getenv("B200C_K1_PAD"); return e ? atoi(e) : 0; }();
-    if (k1_pad > 48 * 1024 - 4096) { static bool once = false; if (!once) { cudaFuncSetAttribute(k_decompress_multi_thr, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); once = true; } }
-    B200C_LAUNCH(c, k_decompress_multi_thr, (unsigned)((total + 127) / 128), 128, (size_t)k1_pad, c->d_tables, d, nseg, total, verify, d_err);
+    unsigned long long* next = (unsigned long long*)(d + nseg);      // chunk counter of the launch (k_decompress_multi_thr)
+    B200C_CUDA_TRY(c, cudaMemsetAsync(next, 0, sizeof(*next), c->stream));
+    B200C_LAUNCH(c, k_decompress_multi_thr, k1_grid(c, total), K1_THREADS, c->k1_smem, c->d_tables, d, nseg, total, verify, d_err, next);
     return B200C_OK;
 }
 
@@ -284,6 +308,9 @@ b200c_ctx* b200c_create(int device, size_t workspace_bytes) {
     b200c_ctx* c = new b200c_ctx();
     c->device = device;
     if (cudaDeviceGetAttribute(&c->nsm, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || c->nsm <= 0) { delete c; return nullptr; }
+    if (cudaDeviceGetAttribute(&c->l2_bytes, cudaDevAttrL2CacheSize, device) != cudaSuccess || c->l2_bytes <= 0) { delete c; return nullptr; }
+    if (cudaDeviceGetAttribute(&c->smem_per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, device) != cudaSuccess ||
+        cudaDeviceGetAttribute(&c->smem_reserved_per_block, cudaDevAttrReservedSharedMemoryPerBlock, device) != cudaSuccess) { delete c; return nullptr; }
     if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) { delete c; return nullptr; }
     cudaEventCreate(&c->ev0); cudaEventCreate(&c->ev1);
     for (auto& e : c->ev_stage) cudaEventCreate(&e);
@@ -300,6 +327,7 @@ b200c_ctx* b200c_create(int device, size_t workspace_bytes) {
     if (cudaMallocHost(&c->h_pinned, c->h_pinned_cap) != cudaSuccess) { cudaFree(c->d_tables); delete c; return nullptr; }
     cudaFuncSetAttribute(k_compress_chunks, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536 + 65536 + 16);
     cudaFuncSetAttribute(k_compress_chunks_snappy_direct, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536);
+    k1_plan(c);
     (void)workspace_bytes;
     return c;
 }
@@ -418,7 +446,7 @@ int b200c_decompress_chunks(b200c_ctx* c, int comp, const uint8_t* data, uint64_
     ChunkErr* d_err; B200C_TRY(ws_typed(c, WSC_ERR, 1, &d_err));
     B200C_CUDA_TRY(c, cudaMemsetAsync(d_err, 0xFF, sizeof(ChunkErr), c->stream));
     timing_begin(c);
-    int rc = decompress_stream_device(c, comp, d_data, data_len, d_offs, nchunks, chunk_len, max_clen, data_length, d_out, verify_crc, d_err, 0, ~0ull, 0);
+    int rc = decompress_stream_device(c, comp, d_data, data_len, d_offs, nchunks, chunk_len, max_clen, data_length, d_out, verify_crc, d_err, 0, ~0ull, 0, nullptr, ~0ull);
     int rc2 = timing_end(c);
     if (rc != B200C_OK) return rc;
     if (rc2 != B200C_OK) return rc2;

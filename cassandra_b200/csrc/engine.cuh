@@ -20,6 +20,9 @@ struct WsBuf { void* p = nullptr; size_t cap = 0; };
 struct b200c_ctx {
     int device = 0;
     int nsm = 0;                                   // SMs of the device: grid-stride kernels launch a fixed number of blocks per SM
+    int l2_bytes = 0;                              // L2 cache of the device: sizes K1's chunks in flight (engine.cu: k1_plan)
+    int smem_per_sm = 0, smem_reserved_per_block = 0;
+    int k1_blocks_per_sm = 1; size_t k1_smem = 0;  // K1 thread kernels: resident blocks per SM and the dynamic shared memory that caps them there
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     b200c::DevTables* d_tables = nullptr;
