@@ -2,8 +2,9 @@
 // data-parallel kernels on one H100:
 //
 //   K1  k_decompress_chunks      every input chunk -> U (CRC verified)                          [codec.cuh]
-//   K2  k_index_find/chain/emit  Index.db walk of BigTableScanner (format/big/BigTableScanner.java:135-184) done speculatively in
-//                                256-byte blocks, proven equal to the sequential parse, + Murmur3 token per key
+//   K2  k_index_walk_count/emit  Index.db walk of BigTableScanner (format/big/BigTableScanner.java:135-184), one thread per Summary.db
+//                                interval, proven equal to the sequential parse, + Murmur3 token per key and the order check
+//                                (without usable samples: k_index_find/chain/emit, speculated in 256-byte blocks and proven the same way)
 //   K3  k_bucket_bounds + k_merge_buckets   the partition-level MergeIterator (S/utils/MergeIterator.java:154-219): token space is
 //                                cut into buckets, one warp per bucket runs a tournament over its <= 64 sources (one or two
 //                                per lane, warp-min by shuffles); equal keys reduce together in source order
@@ -18,6 +19,7 @@
 #include "partition.cuh"
 #include "partition_tile.cuh"
 #include "meta.cuh"
+#include "index_walk.cuh"
 #include <climits>
 #include <vector>
 #include <algorithm>
@@ -40,6 +42,7 @@ int decompress_stream_device(b200c_ctx* c, int comp, const uint8_t* d_data, uint
 int decompress_multi_device(b200c_ctx* c, K1Seg* segs, int nseg, int verify, ChunkErr* d_err, int ws_slot);
 
 enum { IB = 256 };                       // Index.db speculation block
+static_assert(IW_PAD <= 64, "the Index.db workspace keeps 64 bytes behind every input (index_walk.cuh)");
 #ifndef B200C_K4_STAGED_DEFAULT
 #define B200C_K4_STAGED_DEFAULT 0          // flipped to 1 once the staged mapping has beaten the global one in bench.py
 #endif
@@ -62,8 +65,7 @@ __device__ __forceinline__ void report_err(DevErr* e, int kind, int input, uint6
 }
 
 // ---- Murmur3 (Cassandra variant): S/utils/MurmurHash.java:178-260, token = Murmur3Partitioner.getToken :256-296 ---------------
-__host__ __device__ __forceinline__ uint64_t rotl64(uint64_t v, int n) { return (v << n) | (v >> (64 - n)); }
-__host__ __device__ __forceinline__ uint64_t fmix64(uint64_t k) { k ^= k >> 33; k *= 0xff51afd7ed558ccdULL; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ULL; k ^= k >> 33; return k; }
+// (rotl64 / fmix64: index_walk.cuh, whose word-window Murmur3 must equal this one bit for bit)
 __host__ __device__ int64_t murmur3_token(const uint8_t* key, uint32_t len) {
     if (len == 0) return I64_MIN;
     const uint32_t nblocks = len >> 4;
@@ -227,48 +229,111 @@ __global__ void __launch_bounds__(128) k_index_find_anchors(const CParams* __res
     }
 }
 
-// K2 with Summary.db samples, in two walks instead of four passes: every Summary interval (the entries between two samples: 128 by default,
-// ~2 KB of Index.db) is one thread. Walk 1 counts the interval's entries and PROVES the samples: the walk from sample a must land exactly on
-// sample a + 1 (the last one on the end of the slice) and the first sample must be the slice's first byte — by induction the intervals'
-// chains are the sequential parse. Walk 2 (after a scan of the counts) parses again and emits token / key prefix / key length / position.
-// Any interval that does not land marks the input: the call then falls back to the speculate-chain-verify path below, whose sequential
-// last resort reports real damage with its offset.
-__global__ void __launch_bounds__(128) k_index_count_intervals(const CParams* __restrict__ Pp, const uint8_t* __restrict__ IDX, int i, const uint64_t* __restrict__ anchors, uint64_t n,
-                                                               uint64_t bias, uint32_t* __restrict__ acnt, uint32_t* __restrict__ bad) {
-    uint64_t a = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (a >= n) return;
+// K2 with Summary.db samples (the default): every Summary interval (the entries between two samples, 128 by default, ~2 KB of Index.db) of
+// every input is one thread of one launch, and the walk reads Index.db through IdxCursor's window of 16-byte words (index_walk.cuh).
+// Walk 1 counts the interval's entries and PROVES the samples: the walk from sample a must land exactly on sample a + 1 (the last one on the
+// end of the slice) and the first sample must be the slice's first byte, so by induction the intervals' chains are the sequential parse.
+// Walk 2 (after a scan of the counts) parses again, emits token / key prefix / key length / position and checks the order of every adjacent
+// pair: those inside the interval, and the pair across its end (the entry at sample a + 1, where the walk stops, is parsed once more).
+// Any interval that does not land marks its input: the call then runs the speculate-chain-verify path below, whose sequential last resort
+// reports real damage with its offset.
+struct K2Walk {                        // per input: its first interval (over all inputs), its Summary positions in summ[], its slice's file offset
+    uint64_t abase[MAXK + 1], sbase[MAXK], bias[MAXK];
+    int ninputs;
+};
+__device__ __forceinline__ int input_of_interval(const K2Walk& W, uint64_t t) {
+    int lo = 0, hi = W.ninputs - 1;                          // the last input whose first interval is <= t
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (W.abase[mid] <= t) lo = mid; else hi = mid - 1; }
+    return lo;
+}
+// an SSTable is ordered by (token, key) and its partitions do not overlap: tokens must not decrease, equal tokens must come with
+// increasing (8-byte key prefix, length) and Data.db positions must increase along Index.db — everything downstream binary-searches
+// these arrays, so a file in another partitioner's order (or a damaged one) is rejected whatever its size
+// (SortedTableWriter.verifyPartition S/io/sstable/format/SortedTableWriter.java:165-178 enforces the same order when files are written).
+__device__ __forceinline__ bool out_of_order(int64_t tx, uint64_t kx, uint32_t lx, uint64_t ux, int64_t ty, uint64_t ky, uint32_t ly, uint64_t uy) {
+    bool bad = ty < tx || uy <= ux;
+    if (!bad && ty == tx) bad = ky < kx || (ky == kx && lx <= 8 && ly <= lx);
+    return bad;
+}
+__global__ void __launch_bounds__(128) k_index_walk_count(const CParams* __restrict__ Pp, const uint8_t* __restrict__ IDX, const uint64_t* __restrict__ summ,
+                                                          const K2Walk W, uint64_t na, uint32_t* __restrict__ acnt, uint32_t* __restrict__ bad) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= na) return;
     const CParams& P = *Pp;
-    const uint64_t ilen = P.in[i].ilen;
-    uint64_t o = anchors[a] - bias; const uint64_t end = (a + 1 < n) ? anchors[a + 1] - bias : ilen;
+    const int i = input_of_interval(W, t);
+    const InDesc& in = P.in[i];
+    const uint64_t a = t - W.abase[i], n = W.abase[i + 1] - W.abase[i];
+    const uint64_t* anchors = summ + W.sbase[i];
+    uint64_t o = anchors[a] - W.bias[i]; const uint64_t end = (a + 1 < n) ? anchors[a + 1] - W.bias[i] : in.ilen;
+    if ((a == 0 && o != 0) || o >= in.ilen || end > in.ilen || end <= o) { bad[i] = 1; acnt[t] = 0; return; }
+    IdxCursor c; c.init(IDX + in.ibase, in.ilen);
+    IdxEntry e;
     uint32_t cnt = 0;
-    if ((a == 0 && o != 0) || o >= ilen || end > ilen || end <= o) { bad[i] = 1; acnt[a] = 0; return; }
     while (o < end) {
-        uint64_t dpos; uint32_t kl;
-        const uint64_t len = idx_entry(P, IDX, i, o, false, &dpos, &kl);
+        const uint64_t len = iw_entry<false>(c, o, in.ulen, false, e);
         if (!len) break;
         cnt++; o += len;
     }
     if (o != end) bad[i] = 1;
-    acnt[a] = cnt;
+    acnt[t] = cnt;
 }
-__global__ void __launch_bounds__(128) k_index_emit_intervals(const CParams* __restrict__ Pp, const uint8_t* __restrict__ IDX, int i, const uint64_t* __restrict__ anchors, uint64_t n,
-                                                              uint64_t bias, const uint64_t* __restrict__ ascan /* of this input's intervals, [n + 1] */, uint64_t g0,
-                                                              int64_t* __restrict__ tok, uint64_t* __restrict__ kp, uint16_t* __restrict__ klen, uint64_t* __restrict__ upos) {
-    uint64_t a = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (a >= n) return;
+// The lanes of a warp emit entries ~128 apart, so a plain store per entry and array leaves every 32-byte sector of the outputs written in
+// 2..16 pieces at different times; with ~270 K threads in flight those sectors do not stay in L2 between the pieces. Each thread therefore
+// gathers its entries in its own column of shared memory and stores every aligned group that it owns whole (4 entries of the 8-byte arrays,
+// 16 of klen: one 32-byte sector each) with two 16-byte stores; only the groups at the two ends of its interval go out entry by entry.
+enum { EW_THREADS = 128 };
+template <typename T, int G>
+__device__ __forceinline__ void ew_flush(T* __restrict__ out, const T (*s)[EW_THREADS], uint64_t glast, uint64_t gfirst) {
+    const uint64_t gs = glast & ~(uint64_t)(G - 1);
+    if (gs >= gfirst && glast - gs == G - 1) {
+        static_assert(sizeof(T) * G == 32, "one sector per group");
+        alignas(16) T v[G];
+#pragma unroll
+        for (int q = 0; q < G; q++) v[q] = s[q][threadIdx.x];
+        uint4 h0, h1; memcpy(&h0, &v[0], 16); memcpy(&h1, &v[G / 2], 16);
+        uint4* d = (uint4*)(out + gs);                     // (the workspace arrays are 256-byte aligned)
+        d[0] = h0; d[1] = h1;
+    } else for (uint64_t g = gs > gfirst ? gs : gfirst; g <= glast; g++) out[g] = s[g & (G - 1)][threadIdx.x];
+}
+__global__ void __launch_bounds__(EW_THREADS) k_index_walk_emit(const CParams* __restrict__ Pp, const uint8_t* __restrict__ IDX, const uint64_t* __restrict__ summ,
+                                                         const K2Walk W, uint64_t na, const uint64_t* __restrict__ ascan /* [na + 1] */, const uint64_t* __restrict__ pbase,
+                                                         int64_t* __restrict__ tok, uint64_t* __restrict__ kp, uint16_t* __restrict__ klen, uint64_t* __restrict__ upos,
+                                                         DevErr* __restrict__ err) {
+    __shared__ __align__(16) int64_t s_tok[4][EW_THREADS];
+    __shared__ __align__(16) uint64_t s_kp[4][EW_THREADS], s_up[4][EW_THREADS];
+    __shared__ __align__(16) uint16_t s_kl[16][EW_THREADS];
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= na) return;
     const CParams& P = *Pp;
+    const int i = input_of_interval(W, t);
     const InDesc& in = P.in[i];
-    uint64_t o = anchors[a] - bias; const uint64_t end = (a + 1 < n) ? anchors[a + 1] - bias : in.ilen;
-    uint64_t g = g0 + (ascan[a] - ascan[0]); const uint64_t gend = g0 + (ascan[a + 1] - ascan[0]);
+    const uint64_t a = t - W.abase[i], n = W.abase[i + 1] - W.abase[i];
+    const uint64_t* anchors = summ + W.sbase[i];
+    uint64_t o = anchors[a] - W.bias[i]; const uint64_t end = (a + 1 < n) ? anchors[a + 1] - W.bias[i] : in.ilen;
+    const uint64_t s0 = ascan[W.abase[i]];
+    uint64_t g = pbase[i] + (ascan[t] - s0); const uint64_t gfirst = g, gend = pbase[i] + (ascan[t + 1] - s0);
+    const bool murmur = !P.partitioner;
+    IdxCursor c; c.init(IDX + in.ibase, in.ilen);
+    IdxEntry e, prev;
+    bool have_prev = false;
     for (; o < end && g < gend; g++) {
-        uint64_t dpos; uint32_t kl;
-        const uint64_t len = idx_entry(P, IDX, i, o, false, &dpos, &kl);
-        if (!len) return;                                  // (cannot happen: walk 1 parsed the same bytes)
-        const uint8_t* key = IDX + in.ibase + o + 2;
-        uint64_t pre = 0; for (uint32_t q = 0; q < 8; q++) pre = (pre << 8) | (q < kl ? key[q] : 0);
-        tok[g] = P.partitioner ? (int64_t)(pre ^ 0x8000000000000000ull) : murmur3_token(key, kl);       // (see k_index_emit)
-        kp[g] = pre; klen[g] = (uint16_t)kl; upos[g] = in.ubase + dpos;
+        const uint64_t len = iw_entry<true>(c, o, in.ulen, murmur, e);
+        if (!len) break;                                   // (cannot happen: walk 1 parsed the same bytes)
+        // Index.db <-> Data.db consistency is checked by K4 when it parses the partition header (see k_index_emit)
+        s_tok[g & 3][threadIdx.x] = e.tok; s_kp[g & 3][threadIdx.x] = e.pre; s_up[g & 3][threadIdx.x] = in.ubase + e.pos; s_kl[g & 15][threadIdx.x] = (uint16_t)e.kl;
+        if ((g & 3) == 3) { ew_flush<int64_t, 4>(tok, s_tok, g, gfirst); ew_flush<uint64_t, 4>(kp, s_kp, g, gfirst); ew_flush<uint64_t, 4>(upos, s_up, g, gfirst); }
+        if ((g & 15) == 15) ew_flush<uint16_t, 16>(klen, s_kl, g, gfirst);
+        if (have_prev && out_of_order(prev.tok, prev.pre, prev.kl, prev.pos, e.tok, e.pre, e.kl, e.pos)) report_err(err, 3, i, prev.pos);
+        prev = e; have_prev = true;
         o += len;
+    }
+    if (g > gfirst) {                                      // the last group, if it is not whole
+        const uint64_t gl = g - 1;
+        if ((gl & 3) != 3) { ew_flush<int64_t, 4>(tok, s_tok, gl, gfirst); ew_flush<uint64_t, 4>(kp, s_kp, gl, gfirst); ew_flush<uint64_t, 4>(upos, s_up, gl, gfirst); }
+        if ((gl & 15) != 15) ew_flush<uint16_t, 16>(klen, s_kl, gl, gfirst);
+    }
+    if (have_prev && a + 1 < n && o == end) {             // the pair across the interval's end: the first entry of interval a + 1
+        if (iw_entry<true>(c, end, in.ulen, murmur, e) && out_of_order(prev.tok, prev.pre, prev.kl, prev.pos, e.tok, e.pre, e.kl, e.pos)) report_err(err, 3, i, prev.pos);
     }
 }
 
@@ -382,10 +447,7 @@ __global__ void k_input_ranges(const CParams* __restrict__ Pp, const uint64_t* _
     if (range_bytes && hi > lo) atomicAdd(range_bytes, (unsigned long long)(upos[pbase[i] + hi] - upos[pbase[i] + lo]));
 }
 
-// an SSTable is ordered by (token, key) and its partitions do not overlap: tokens must not decrease, equal tokens must come with
-// increasing (8-byte key prefix, length) and Data.db positions must increase along Index.db — everything downstream binary-searches
-// these arrays, so a file in another partitioner's order (or a damaged one) is rejected here whatever its size
-// (SortedTableWriter.verifyPartition S/io/sstable/format/SortedTableWriter.java:165-178 enforces the same order when files are written).
+// the order check (out_of_order) over all adjacent pairs, for the speculate-chain-verify path
 __global__ void __launch_bounds__(256) k_check_order(const CParams* __restrict__ Pp, const uint64_t* __restrict__ pbase, const uint64_t* __restrict__ pcount,
                                                      const int64_t* __restrict__ tok, const uint64_t* __restrict__ kp, const uint16_t* __restrict__ klen,
                                                      const uint64_t* __restrict__ upos, DevErr* __restrict__ err) {
@@ -394,9 +456,7 @@ __global__ void __launch_bounds__(256) k_check_order(const CParams* __restrict__
         const uint64_t n = pcount[i], b = pbase[i];
         for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g + 1 < n; g += (uint64_t)gridDim.x * blockDim.x) {
             const uint64_t x = b + g, y = x + 1;
-            bool bad = tok[y] < tok[x] || upos[y] <= upos[x];
-            if (!bad && tok[y] == tok[x]) bad = kp[y] < kp[x] || (kp[y] == kp[x] && klen[x] <= 8 && klen[y] <= klen[x]);
-            if (bad) report_err(err, 3, i, upos[x] - P.in[i].ubase);
+            if (out_of_order(tok[x], kp[x], klen[x], upos[x], tok[y], kp[y], klen[y], upos[y])) report_err(err, 3, i, upos[x] - P.in[i].ubase);
         }
     }
 }
@@ -982,7 +1042,7 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         if (in.compressor != COMP_LZ4 && !comp_is_snappy(in.compressor) && in.compressor != COMP_NONE) { c->err = "unknown compressor"; return B200C_EINVAL; }
         ubase[i] = uo; uo += (in.data_length + 64 + 65535) & ~65535ull;
         const uint64_t ilen_i = isl[i].hi - isl[i].lo;               // Index.db bytes this call reads from input i
-        ibase[i] = io; io += (ilen_i + 64 + 255) & ~255ull;
+        ibase[i] = io; io += (ilen_i + 64 + 255) & ~255ull;       // 256-aligned, >= 64 bytes behind every input: K2's 16-byte reads need IW_PAD
         cbase[i] = co; co += (in.data_len + 64 + 255) & ~255ull;
         obase[i] = oo; oo += in.nchunks + 1;
         bbase[i] = bo; bo += (ilen_i + IB - 1) / IB;
@@ -1361,26 +1421,31 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
             B200C_CUDA_TRY(c, cudaMemcpyAsync(d_pcount, pcount.data(), K * 8, cudaMemcpyHostToDevice, st));
             return B200C_OK;
         };
-        // ---- B200C_K2_INTERVALS=1 (A/B; slower than the default on an earlier GPU, not re-measured on the H100 — a thread's 2 KB serial walk, twice, against the
-        //      256-byte blocks of the default path): one thread per Summary interval, count + prove, scan, emit -----------------------------
+        // ---- with Summary.db samples: one thread per Summary interval of every input, count + prove, scan, emit + order check (k_index_walk_*).
+        //      B200C_K2_LEGACY=1 (A/B) runs the speculate-chain-verify path below instead, which also serves inputs without samples, samples
+        //      sparser than 64 KiB per interval (one thread's serial walk would be too long) and any input whose samples did not prove.
+        //      (B200C_K2_INTERVALS=1, which selected the walk by interval while it was not the default, is accepted and changes nothing.)
         bool emitted = false;
-        const bool k2_intervals = getenv("B200C_K2_INTERVALS") != nullptr;
-        bool intervals_ok = have_summaries && k2_intervals;
-        for (int i = 0; i < K && intervals_ok; i++)      // (sparse samples: an interval is one thread's serial walk — leave those to the block-parallel path)
+        const bool k2_legacy = getenv("B200C_K2_LEGACY") != nullptr;
+        bool intervals_ok = have_summaries && !k2_legacy;
+        for (int i = 0; i < K && intervals_ok; i++)
             if (sl[i].hi > sl[i].lo && (!sl[i].s_count || (sl[i].hi - sl[i].lo) / sl[i].s_count > (64u << 10))) intervals_ok = false;
         if (intervals_ok) {
-            std::vector<uint64_t> abase(K + 1, 0);
-            for (int i = 0; i < K; i++) abase[i + 1] = abase[i] + sl[i].s_count;
-            const uint64_t na = abase[K];
+            K2Walk W; memset(&W, 0, sizeof(W));
+            W.ninputs = K;
+            for (int i = 0; i < K; i++) { W.abase[i + 1] = W.abase[i] + sl[i].s_count; W.sbase[i] = sb[i]; W.bias[i] = sl[i].lo; }
+            const uint64_t na = W.abase[K];
             uint32_t *d_acnt, *d_abad; uint64_t* d_ascan;
             B200C_TRY(ws_typed(c, WS_ICNT, na + 1, &d_acnt));
             B200C_TRY(ws_typed(c, WS_ISCAN, na + 2, &d_ascan));
             B200C_TRY(ws_typed(c, WS_IBAD, (size_t)K + 1, &d_abad));
             B200C_CUDA_TRY(c, cudaMemsetAsync(d_abad, 0, (K + 1) * 4, st));
-            for (int i = 0; i < K; i++) if (sl[i].s_count)
-                B200C_LAUNCH(c, k_index_count_intervals, (unsigned)((sl[i].s_count + 127) / 128), 128, 0, dP, IDX, i, d_summ + sb[i], sl[i].s_count, sl[i].lo, d_acnt + abase[i], d_abad);
-            if (na) B200C_TRY(exclusive_scan<uint32_t>(c, d_acnt, na, d_ascan, WS_SCANA, 0)); else B200C_CUDA_TRY(c, cudaMemsetAsync(d_ascan, 0, 16, st));
-            for (int i = 0; i <= K; i++) B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 8 + i, d_ascan + abase[i], 8, cudaMemcpyDeviceToHost, st));
+            const unsigned grid = (unsigned)((na + EW_THREADS - 1) / EW_THREADS);
+            if (na) {
+                B200C_LAUNCH(c, k_index_walk_count, grid, EW_THREADS, 0, dP, IDX, d_summ, W, na, d_acnt, d_abad);
+                B200C_TRY(exclusive_scan<uint32_t>(c, d_acnt, na, d_ascan, WS_SCANA, 0));
+            } else B200C_CUDA_TRY(c, cudaMemsetAsync(d_ascan, 0, 16, st));
+            for (int i = 0; i <= K; i++) B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 8 + i, d_ascan + W.abase[i], 8, cudaMemcpyDeviceToHost, st));
             B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_cerr, 8, cudaMemcpyDeviceToHost, st));
             B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 300, d_abad, (K + 1) * 4, cudaMemcpyDeviceToHost, st));
             B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
@@ -1392,9 +1457,7 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
                 for (int i = 0; i < K; i++) { pcount[i] = h[8 + i + 1] - h[8 + i]; pbase[i] = total_parts; total_parts += pcount[i] + 1; }
                 pbase[K] = total_parts;
                 B200C_TRY(alloc_arrays());
-                for (int i = 0; i < K; i++) if (sl[i].s_count)
-                    B200C_LAUNCH(c, k_index_emit_intervals, (unsigned)((sl[i].s_count + 127) / 128), 128, 0, dP, IDX, i, d_summ + sb[i], sl[i].s_count, sl[i].lo, d_ascan + abase[i], pbase[i],
-                                 d_tok, d_kp, d_klen, d_upos);
+                if (na) B200C_LAUNCH(c, k_index_walk_emit, grid, EW_THREADS, 0, dP, IDX, d_summ, W, na, d_ascan, d_pbase, d_tok, d_kp, d_klen, d_upos, d_err);
                 emitted = true;
             }
         }
@@ -1446,8 +1509,8 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         B200C_TRY(alloc_arrays());
         if (nblocks) B200C_LAUNCH(c, k_index_emit, (unsigned)((nblocks + 255) / 256), 256, 0, dP, IDX, d_bbase, nblocks, d_istart, d_icnt, d_iscan, d_pbase,
                                   d_tok, d_kp, d_klen, d_upos, d_err);
-        }      // (legacy path)
         if (total_parts > (uint64_t)K) B200C_LAUNCH(c, k_check_order, 8 * c->nsm, 256, 0, dP, d_pbase, d_pcount, d_tok, d_kp, d_klen, d_upos, d_err);
+        }      // (speculate-chain-verify path; the walk by interval checks the order as it emits)
         B200C_LAUNCH(c, k_input_ranges, (K + 63) / 64, 64, 0, dP, d_pbase, d_pcount, d_tok, d_upos, tlo, thi, d_range, d_rbytes);
         B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_range, 2 * K * 8, cudaMemcpyDeviceToHost, st));
         B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 200, d_err, 8, cudaMemcpyDeviceToHost, st));
