@@ -275,6 +275,81 @@ __global__ void k_digest_final(const DevTables* __restrict__ T, const uint64_t* 
     acc[1] = ~(acc[0] ^ gf2_mulmod(0xFFFFFFFFu, gf2_xpow8n(T, total)));
 }
 
+// ---- uncompressed Data.db + CRC.db: K1 ingest (verify, copy into U) and K5 checksum (copy out, CRC per chunk) -----------------------
+// ChecksummedSequentialWriter (S/io/util/ChecksummedSequentialWriter.java) writes Data.db as it is, and CRC.db as the BE i32 chunk size
+// followed by one BE i32 CRC32 per chunk (ChecksumWriter.appendDirect, S/io/util/ChecksumWriter.java:62-89). Each chunk is streamed once by
+// one block: its warps cut it into contiguous segments of whole 512-byte rows, lane l loads (and stores) the aligned 16-byte words
+// l, l + 32, ... of its warp's segment, folds each word with slice-by-4 and advances its register by one row (crc_adv512) per step. The
+// lane registers are shifted to the segment's end (xp_lane16) and XOR-reduced, the segments to the chunk's end (x^(8n)).
+__device__ __forceinline__ uint32_t crc_step4(const uint32_t (*t)[256], uint32_t x) {
+    return t[3][x & 0xff] ^ t[2][(x >> 8) & 0xff] ^ t[1][(x >> 16) & 0xff] ^ t[0][x >> 24];
+}
+__device__ __forceinline__ void raw_chunks_block(const DevTables* __restrict__ T, const RawArgs& a) {
+    __shared__ uint32_t s_crc[4][256], s_adv[4][256], s_xl[32], s_part[RAW_WARPS];
+    for (int i = threadIdx.x; i < 1024; i += RAW_THREADS) { s_crc[i >> 8][i & 255] = T->crc_t[i >> 8][i & 255]; s_adv[i >> 8][i & 255] = T->crc_adv512[i >> 8][i & 255]; }
+    if (threadIdx.x < 32) s_xl[threadIdx.x] = T->xp_lane16[threadIdx.x];
+    __syncthreads();
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    for (uint64_t chunk = a.chunk0 + blockIdx.x; chunk < a.chunk_end; chunk += gridDim.x) {
+        const uint64_t start = chunk * (uint64_t)a.L;
+        const uint32_t len = (uint32_t)min((uint64_t)a.L, a.n - start);
+        const uint8_t* src = a.src + start; uint8_t* dst = a.dst ? a.dst + start : nullptr;
+        // 16-byte words from the first aligned address of the chunk on (a file of an LCS output starts wherever its first partition does);
+        // the bytes before it and behind the last whole word go byte by byte below. A destination must share the source's alignment.
+        const uint32_t head = min(len, (uint32_t)((16 - ((uintptr_t)src & 15)) & 15));
+        const bool vec = !dst || ((((uintptr_t)src) ^ ((uintptr_t)dst)) & 15) == 0;
+        const uint32_t nbody = vec ? (len - head) & ~15u : 0;      // bytes taken as 16-byte words
+        if (vec) {
+            const uint32_t nw = nbody >> 4, rows = (nw + 31) >> 5, rpw = (rows + RAW_WARPS - 1) / RAW_WARPS;
+            const uint32_t wb = min(nw, wid * rpw * 32), we = min(nw, (wid + 1) * rpw * 32), sw = we - wb;
+            const uint4* s4 = (const uint4*)(src + head) + wb; uint4* d4 = dst ? (uint4*)(dst + head) + wb : nullptr;
+            const int pad = (int)((32 - (sw & 31)) & 31), nrow = (int)((sw + pad) >> 5);     // virtual leading zero words: whole rows
+            uint32_t u = 0;
+#pragma unroll 4
+            for (int k = 0; k < nrow; k++) {
+                const int idx = k * 32 + lane - pad;
+                uint32_t s = 0;
+                if (idx >= 0) {
+                    const uint4 v = s4[idx];
+                    if (d4) d4[idx] = v;
+                    s = crc_step4(s_crc, v.x); s = crc_step4(s_crc, s ^ v.y); s = crc_step4(s_crc, s ^ v.z); s = crc_step4(s_crc, s ^ v.w);
+                }
+                u = crc_adv128(s_adv, u) ^ s;
+            }
+            uint32_t r = gf2_mulmod(u, s_xl[lane]);
+#pragma unroll
+            for (int d = 16; d; d >>= 1) r ^= __shfl_xor_sync(FULL_MASK, r, d);
+            if (lane == 0) s_part[wid] = (r && nbody > we * 16) ? gf2_mulmod(r, gf2_xpow8n(T, nbody - we * 16)) : r;
+        } else {                                                    // source and destination aligned differently: bytes
+            if (dst) for (uint32_t i = threadIdx.x; i < len; i += RAW_THREADS) dst[i] = src[i];
+            if (wid == 0) { const uint32_t r = warp_crc32_raw(T, T->crc_adv128, src, (int)len, lane); if (lane == 0) s_part[0] = r; }
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            uint32_t raw = s_part[0];
+            if (vec) {
+                uint32_t body = s_part[0];
+                for (int w = 1; w < RAW_WARPS; w++) body ^= s_part[w];
+                raw = 0;                                            // register(head || body) = register(head) * x^(8 |body|) ^ register(body)
+                for (uint32_t i = 0; i < head; i++) { const uint8_t b = src[i]; raw = s_crc[0][(raw ^ b) & 0xff] ^ (raw >> 8); if (dst) dst[i] = b; }
+                if (raw && nbody) raw = gf2_mulmod(raw, gf2_xpow8n(T, nbody));
+                raw ^= body;
+                for (uint32_t i = head + nbody; i < len; i++) { const uint8_t b = src[i]; raw = s_crc[0][(raw ^ b) & 0xff] ^ (raw >> 8); if (dst) dst[i] = b; }
+            }
+            const uint32_t crc = ~(raw ^ gf2_mulmod(0xFFFFFFFFu, gf2_xpow8n(T, len)));
+            if (a.crc_out) a.crc_out[chunk] = crc;
+            if (a.seg_raw) a.seg_raw[chunk] = raw;
+            if (a.ends) { a.ends[chunk + 1] = a.ebase + start + len; if (chunk == 0) a.ends[0] = a.ebase; }
+            if (a.crc_exp && a.crc_exp[chunk] != (uint64_t)crc) report_chunk_err(a.err, ((uint64_t)a.tag << 40) | chunk, 1);
+        }
+        __syncthreads();
+    }
+}
+// K1 of an uncompressed input: verify every chunk against CRC.db, copy it into U unless it was copied there from the host
+__global__ void __launch_bounds__(RAW_THREADS, 8) k_raw_ingest(const DevTables* __restrict__ T, const RawArgs a) { raw_chunks_block(T, a); }
+// K5 of an uncompressed output: the CRC.db entry and digest register of every chunk, the bytes copied out when a destination is given
+__global__ void __launch_bounds__(RAW_THREADS, 8) k_raw_checksum(const DevTables* __restrict__ T, const RawArgs a) { raw_chunks_block(T, a); }
+
 // ---- K1: CRC verify + decompress ----------------------------------------------------------------------------------
 // One warp per chunk, two chunks per block, NO shared-memory image: literals and matches are written straight to the output
 // stream in global memory and match sources are read back from it (a warp may read what its other lanes stored after

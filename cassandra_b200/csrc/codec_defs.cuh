@@ -6,6 +6,8 @@
 namespace b200c {
 
 enum { COMP_NONE = 0, COMP_LZ4 = 1, COMP_SNAPPY = 2, COMP_SNAPPY15 = 3 };      // SNAPPY15: hash table of up to 2^15 entries (snappy >= 1.2.0)
+// compression disabled: Data.db is the uncompressed stream and the chunk table holds CRC.db's per-chunk CRC32s (include/b200c.h)
+enum { COMP_UNCOMPRESSED = 4 };
 __host__ __device__ __forceinline__ bool comp_is_snappy(int c) { return c == COMP_SNAPPY || c == COMP_SNAPPY15; }
 
 __host__ __device__ __forceinline__ int chunk_max_compressed(int comp, int chunk_len) {
@@ -29,5 +31,18 @@ struct K1Seg { const uint8_t* data; uint64_t data_len; const uint64_t* offs; uin
                uint64_t chunk0, count, first; int chunk_len, max_clen, tag, _pad;
                uint64_t rec0, rec_span;         // two-pass LZ4 (lz4_batch.cuh): first record slot of this segment, compressed bytes its slots were sized for
                const uint8_t* tail; uint64_t tail_off; };     // staged copy of the file's bytes from tail_off on (k1_src)
+
+// one launch of the uncompressed-stream kernels (codec.cuh: k_raw_ingest / k_raw_checksum)
+enum { RAW_WARPS = 8, RAW_THREADS = 32 * RAW_WARPS };
+struct RawArgs {
+    const uint8_t* src; uint8_t* dst;       // dst: null = nothing stored (verify in place, checksum only)
+    uint64_t n; int L, tag;                 // stream bytes, chunk length, input number of error reports
+    uint64_t chunk0, chunk_end;             // chunks [chunk0, chunk_end) of the stream
+    const uint64_t* crc_exp;                // K1: CRC.db entries to verify against (kind 1 on a mismatch)
+    uint64_t* crc_out;                      // K5: CRC.db entries, zero-extended
+    uint32_t* seg_raw;                      // K5: zero-init CRC register of each chunk (k_digest)
+    uint64_t* ends; uint64_t ebase;         // K5: ends[c + 1] = ebase + end of chunk c and ends[0] = ebase (k_digest's offsets)
+    ChunkErr* err;
+};
 
 } // namespace b200c

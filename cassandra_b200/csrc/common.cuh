@@ -15,6 +15,8 @@ struct DevTables {
     uint32_t crc_adv128[4][256]; // advance a CRC register through 128 zero bytes, byte-sliced
     uint32_t xp_lane[32];        // x^(8*4*(32-l)) mod P  (reflected)
     uint32_t xp_pow2[64];        // x^(8*2^k) mod P
+    uint32_t crc_adv512[4][256]; // advance a CRC register through 512 zero bytes (one warp row of 16-byte words), byte-sliced
+    uint32_t xp_lane16[32];      // x^(8*16*(31-l)) mod P: bytes behind lane l's 16-byte word in a 512-byte row
 };
 
 __host__ __device__ __forceinline__ uint32_t gf2_mulmod(uint32_t a, uint32_t b) {

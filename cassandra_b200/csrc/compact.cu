@@ -40,6 +40,8 @@ int decompress_stream_device(b200c_ctx* c, int comp, const uint8_t* d_data, uint
                              int chunk_len, int max_clen, uint64_t data_length, uint8_t* d_out, int verify, ChunkErr* d_err, uint64_t chunk0, uint64_t count, int tag,
                              const uint8_t* tail, uint64_t tail_off);
 int decompress_multi_device(b200c_ctx* c, K1Seg* segs, int nseg, int verify, ChunkErr* d_err, int ws_slot);
+int raw_chunks_device(b200c_ctx* c, bool ingest, const RawArgs& a);
+int raw_stream_device(b200c_ctx* c, const uint8_t* d_in, uint64_t n, int chunk_len, uint8_t* d_out, uint64_t* d_crc, uint32_t* digest, int ws_base);
 
 enum { IB = 256 };                       // Index.db speculation block
 static_assert(IW_PAD <= 64, "the Index.db workspace keeps 64 bytes behind every input (index_walk.cuh)");
@@ -961,6 +963,14 @@ __global__ void k_find_cut(const uint64_t* __restrict__ dpos, uint64_t jlo, uint
     uint64_t full = flushed(dpos[a] - start_b);
     out[1] = full > nwin ? 2 : 0;
 }
+// the same for an uncompressed output: getEstimatedOnDiskBytesWritten() is position(), which counts the bytes still buffered
+// (S/io/util/SequentialWriter.java:304-312,342-345), so the writer switches before the first partition that starts more than `limit` bytes
+// into the file: the file ends after the partition that took it past the limit
+__global__ void k_find_cut_raw(const uint64_t* __restrict__ dpos, uint64_t jlo, uint64_t nparts, uint64_t start_b, uint64_t limit, uint64_t* __restrict__ out) {
+    uint64_t a = jlo + 1, b = nparts;
+    while (a < b) { const uint64_t mid = (a + b) / 2; if (dpos[mid] - start_b > limit) b = mid; else a = mid + 1; }
+    out[0] = a;
+}
 __global__ void __launch_bounds__(256) k_rel_pos(const uint64_t* __restrict__ dpos, uint64_t jlo, uint64_t jhi, uint64_t start_b, uint64_t* __restrict__ dposf) {
     uint64_t j = jlo + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j <= jhi) dposf[j] = dpos[j] - start_b;
@@ -1033,17 +1043,20 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
     std::vector<uint64_t> ubase(K + 1), ibase(K + 1), cbase(K + 1), obase(K + 1), bbase(K + 1);
     CParams hp; memset(&hp, 0, sizeof(hp));
     std::vector<InDesc> hin(K); memset(hin.data(), 0, sizeof(InDesc) * K);
-    uint64_t uo = 0, io = 0, co = 0, oo = 0, bo = 0;
+    uint64_t uo = 0, io = 0, co = 0, oo = 0, bo = 0, in_bytes = 0;
     for (int i = 0; i < K; i++) {
         const b200c_input& in = m->inputs[i];
         if (in.chunk_len <= 0 || in.chunk_len > 65536 || (in.chunk_len & (in.chunk_len - 1))) { c->err = "input chunk_len"; return B200C_EUNSUPPORTED; }
         if (in.ncolumns < 0 || in.ncolumns >= 64) { c->err = "input columns"; return B200C_EUNSUPPORTED; }
         if (in.nchunks != (in.data_length + in.chunk_len - 1) / (uint64_t)in.chunk_len) { c->err = "chunk count does not match data_length"; return B200C_EINVAL; }
-        if (in.compressor != COMP_LZ4 && !comp_is_snappy(in.compressor) && in.compressor != COMP_NONE) { c->err = "unknown compressor"; return B200C_EINVAL; }
+        if (in.compressor != COMP_LZ4 && !comp_is_snappy(in.compressor) && in.compressor != COMP_NONE && in.compressor != COMP_UNCOMPRESSED) { c->err = "unknown compressor"; return B200C_EINVAL; }
+        if (in.compressor == COMP_UNCOMPRESSED && in.data_len != in.data_length) { c->err = "uncompressed input: data_length must equal data_len"; return B200C_EINVAL; }
         ubase[i] = uo; uo += (in.data_length + 64 + 65535) & ~65535ull;
         const uint64_t ilen_i = isl[i].hi - isl[i].lo;               // Index.db bytes this call reads from input i
         ibase[i] = io; io += (ilen_i + 64 + 255) & ~255ull;       // 256-aligned, >= 64 bytes behind every input: K2's 16-byte reads need IW_PAD
-        cbase[i] = co; co += (in.data_len + 64 + 255) & ~255ull;
+        // uncompressed inputs are copied from the host straight into U (no staging in CD); `in_bytes` counts every input for the piece schedule
+        cbase[i] = co; if (in.compressor != COMP_UNCOMPRESSED) co += (in.data_len + 64 + 255) & ~255ull;
+        in_bytes += (in.data_len + 64 + 255) & ~255ull;
         obase[i] = oo; oo += in.nchunks + 1;
         bbase[i] = bo; bo += (ilen_i + IB - 1) / IB;
         InDesc& d = hin[i];
@@ -1099,16 +1112,16 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         if (const char* e = getenv("B200C_RANGES")) {
             int n = std::max(1, std::min((int)MAX_RANGES, atoi(e))); forced_ranges = true;
             for (int r = 1; r < n; r++) cuts.push_back((double)r / n);
-        } else if (co >= (1536ull << 20)) {
+        } else if (in_bytes >= (1536ull << 20)) {
             // The kernels of a piece take longer than its copies, so the pipeline is kernel bound as long as no piece waits for its own
             // data: a small first piece (the kernels start early), then EQUAL pieces. Doubling pieces (B200C_SCHEDULE=geometric) end with a
             // piece of half the input that cannot start before the last byte has arrived, and the kernels idle until it has.
-            const double f0 = std::min(0.5, std::max(1.0 / 16, (double)(512ull << 20) / (double)co));
+            const double f0 = std::min(0.5, std::max(1.0 / 16, (double)(512ull << 20) / (double)in_bytes));
             const char* sch = getenv("B200C_SCHEDULE");
             if (sch && !strcmp(sch, "geometric")) { for (double f = f0; f < 1.0 && cuts.size() + 1 < MAX_RANGES; f *= 2) cuts.push_back(f); }
             else {
-                const double piece = std::max((double)co / 8, (double)(768ull << 20));
-                int n = (int)std::ceil((1.0 - f0) * (double)co / piece); n = std::max(1, std::min(n, (int)MAX_RANGES - 1));
+                const double piece = std::max((double)in_bytes / 8, (double)(768ull << 20));
+                int n = (int)std::ceil((1.0 - f0) * (double)in_bytes / piece); n = std::max(1, std::min(n, (int)MAX_RANGES - 1));
                 for (int k = 0; k < n; k++) cuts.push_back(f0 + (1.0 - f0) * k / n);
             }
         }
@@ -1167,24 +1180,26 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
     const int nr = (int)T.size() - 1;
     uint8_t *U, *CD, *IDX; uint64_t* CO; CParams* dP; uint64_t* d_bbase; DevErr* d_err; ChunkErr* d_cerr; RunStats* d_stats; unsigned long long* d_hist;
     B200C_TRY(ws_typed(c, WS_U, uo + 64, &U));
-    // K1's view of input i. Host inputs are staged in CD / CO. Device-resident inputs are read where the caller keeps them: no copy,
+    // K1's view of input i. Host inputs are staged in CD / CO (uncompressed ones go to U itself and are verified there). Device-resident inputs are read where the caller keeps them: no copy,
     // no second image of the compressed inputs in device memory; only the file's tail is staged for the decoders' word reads (k1_src).
     std::vector<const uint8_t*> k1_data(K), k1_tail(K, nullptr); std::vector<const uint64_t*> k1_offs(K); std::vector<uint64_t> k1_tail_off(K, ~0ull);
     if (dev) {
         std::vector<uint64_t> tb(K + 1, 0);
-        for (int i = 0; i < K; i++) tb[i + 1] = tb[i] + ((std::min(m->inputs[i].data_len, k1_tail_window(chunk_max_compressed(m->inputs[i].compressor, m->inputs[i].chunk_len), m->inputs[i].chunk_len)) + 64 + 15) & ~15ull);
+        // (uncompressed inputs: the ingest kernel reads whole aligned words inside the file only, nothing to stage)
+        auto tail_window = [&](const b200c_input& in) -> uint64_t { return in.compressor == COMP_UNCOMPRESSED ? 0 : std::min(in.data_len, k1_tail_window(chunk_max_compressed(in.compressor, in.chunk_len), in.chunk_len)); };
+        for (int i = 0; i < K; i++) tb[i + 1] = tb[i] + ((tail_window(m->inputs[i]) + 64 + 15) & ~15ull);
         uint8_t* TAIL; B200C_TRY(ws_typed(c, WS_K1TAIL, tb[K] + 64, &TAIL));
         CD = nullptr; CO = nullptr;
         for (int i = 0; i < K; i++) {
             const b200c_input& in = m->inputs[i];
-            const uint64_t win = std::min(in.data_len, k1_tail_window(chunk_max_compressed(in.compressor, in.chunk_len), in.chunk_len));
+            const uint64_t win = tail_window(in);
             k1_data[i] = in.data; k1_offs[i] = in.chunk_offsets; k1_tail[i] = TAIL + tb[i]; k1_tail_off[i] = in.data_len - win;
             if (win) B200C_CUDA_TRY(c, cudaMemcpyAsync(TAIL + tb[i], in.data + (in.data_len - win), win, cudaMemcpyDeviceToDevice, c->stream));
         }
     } else {
         B200C_TRY(ws_typed(c, WS_CD, co + 64, &CD));
         B200C_TRY(ws_typed(c, WS_CO, oo + 1, &CO));
-        for (int i = 0; i < K; i++) { k1_data[i] = CD + cbase[i]; k1_offs[i] = CO + obase[i]; }
+        for (int i = 0; i < K; i++) { k1_data[i] = m->inputs[i].compressor == COMP_UNCOMPRESSED ? U + ubase[i] : CD + cbase[i]; k1_offs[i] = CO + obase[i]; }
     }
     B200C_TRY(ws_typed(c, WS_IDX, io + 64, &IDX));
     // Summary.db positions on the device: one run per piece and input (file offsets; K2 subtracts the slice start — no kernel rides on the copy stream)
@@ -1244,13 +1259,20 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         if (m->inputs[i].nchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(co_host[i].data(), m->inputs[i].chunk_offsets, m->inputs[i].nchunks * 8, cudaMemcpyDeviceToHost, cs));
     }
     if (!co_host.empty()) B200C_CUDA_TRY(c, cudaStreamSynchronize(cs));
-    auto chunk_off = [&](int i, uint64_t ch) -> uint64_t { const b200c_input& in = m->inputs[i]; return ch >= in.nchunks ? in.data_len : (co_host.empty() ? in.chunk_offsets[ch] : co_host[i][ch]); };
-    auto copy_chunks = [&](int i, uint64_t a, uint64_t b) -> int {      // compressed bytes of chunks [a, b) of input i -> CD (host inputs)
+    // file offset of chunk ch of input i (an uncompressed input's chunk i sits at i * chunk_len; its chunk table holds CRCs)
+    auto chunk_off = [&](int i, uint64_t ch) -> uint64_t {
+        const b200c_input& in = m->inputs[i];
+        if (ch >= in.nchunks) return in.data_len;
+        if (in.compressor == COMP_UNCOMPRESSED) return ch * (uint64_t)in.chunk_len;
+        return co_host.empty() ? in.chunk_offsets[ch] : co_host[i][ch];
+    };
+    auto copy_chunks = [&](int i, uint64_t a, uint64_t b) -> int {      // compressed bytes of chunks [a, b) of input i -> CD (host inputs; uncompressed -> U)
         const b200c_input& in = m->inputs[i];
         if (a >= b || dev) return B200C_OK;
         uint64_t lo = chunk_off(i, a), hi = chunk_off(i, b);
         if (lo > hi || hi > in.data_len) { c->err = "chunk offsets of input " + std::to_string(i) + " are not increasing"; res->corruption.input = i; res->corruption.kind = 2; res->corruption.chunk = a; res->corruption.offset = 0; return B200C_ECORRUPT; }
-        if (hi > lo) B200C_CUDA_TRY(c, cudaMemcpyAsync(CD + cbase[i] + lo, in.data + lo, hi - lo, kind, cs));
+        uint8_t* const to = in.compressor == COMP_UNCOMPRESSED ? U + ubase[i] : CD + cbase[i];
+        if (hi > lo) B200C_CUDA_TRY(c, cudaMemcpyAsync(to + lo, in.data + lo, hi - lo, kind, cs));
         return B200C_OK;
     };
     // what each piece needs from each input: chunks to copy (deferred mode) and to decompress
@@ -1272,7 +1294,7 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
     };
     for (int i = 0; i < K; i++) {
         const b200c_input& in = m->inputs[i];
-        if (!dev && !deferred && in.data_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(CD + cbase[i], in.data, in.data_len, kind, cs));
+        if (!dev && !deferred && in.data_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(in.compressor == COMP_UNCOMPRESSED ? U + ubase[i] : CD + cbase[i], in.data, in.data_len, kind, cs));
         if (!dev && in.nchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(CO + obase[i], in.chunk_offsets, in.nchunks * 8, kind, cs));
         if (!istream) {
             if (isl[i].hi > isl[i].lo) B200C_CUDA_TRY(c, cudaMemcpyAsync(IDX + ibase[i], in.index + isl[i].lo, isl[i].hi - isl[i].lo, kind, cs));
@@ -1332,6 +1354,12 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
     auto k1 = [&](int i, uint64_t a, uint64_t b) -> int {           // chunks [a, b) of input i
         const b200c_input& in = m->inputs[i];
         if (a >= b) return B200C_OK;
+        if (in.compressor == COMP_UNCOMPRESSED) {          // verify against CRC.db; device-resident inputs are copied into U on the way
+            RawArgs ra; memset(&ra, 0, sizeof(ra));
+            ra.src = k1_data[i]; ra.dst = dev ? U + ubase[i] : nullptr; ra.n = in.data_len; ra.L = in.chunk_len; ra.tag = i;
+            ra.chunk0 = a; ra.chunk_end = std::min(b, in.nchunks); ra.crc_exp = k1_offs[i]; ra.err = d_cerr;
+            return raw_chunks_device(c, true, ra);
+        }
         return decompress_stream_device(c, in.compressor, k1_data[i], in.data_len, k1_offs[i], in.nchunks, in.chunk_len,
                                         in.max_compressed_len, in.data_length, U + ubase[i], 1, d_cerr, a, b - a, i, k1_tail[i], k1_tail_off[i]);
     };
@@ -1376,7 +1404,9 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
     auto check_cancel = [&]() -> int { if (c->cancel.exchange(0)) { c->err = "cancelled"; cudaStreamSynchronize(st); timing_end(c); return B200C_ECANCELLED; } return B200C_OK; };
     auto chunk_error = [&](uint64_t word) -> int {                  // word = d_cerr: (input << 48 | chunk << 8 | kind)
         int which = (int)(word >> 48), kindc = (int)(word & 0xff); uint64_t chunk = (word >> 8) & 0xFFFFFFFFFFull;
-        res->corruption.input = which; res->corruption.kind = kindc; res->corruption.chunk = chunk; res->corruption.offset = 0;
+        // an uncompressed input's chunk starts at chunk * chunk_len of Data.db
+        const uint64_t off = which < K && m->inputs[which].compressor == COMP_UNCOMPRESSED ? chunk * (uint64_t)m->inputs[which].chunk_len : 0;
+        res->corruption.input = which; res->corruption.kind = kindc; res->corruption.chunk = chunk; res->corruption.offset = off;
         c->err = std::string(kindc == 1 ? "chunk CRC mismatch" : "malformed compressed chunk") + " in input " + std::to_string(which) + " chunk " + std::to_string(chunk);
         timing_end(c);
         return B200C_ECORRUPT;
@@ -1563,7 +1593,8 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
     OutStream os;
     // B200C_K5_OVERLAP=1 (A/B; no gain on an earlier GPU, not re-measured on the H100; K4 and K5 are both bound by shared memory and latency, the
     // time K5 spends under the next piece's K1..K3 comes back as slower K2..K4): K5 of piece r on its own stream instead of the main one
-    const bool k5_async = to_host_stream && nr > 1 && []() { const char* e = getenv("B200C_K5_OVERLAP"); return e ? atoi(e) != 0 : false; }();
+    const bool raw_out = m->out_compressor == COMP_UNCOMPRESSED;       // compression disabled: Data.db + CRC.db (k_raw_checksum)
+    const bool k5_async = to_host_stream && nr > 1 && !raw_out && []() { const char* e = getenv("B200C_K5_OVERLAP"); return e ? atoi(e) != 0 : false; }();
     int k5_last = -1;
     if (to_host_stream) B200C_TRY(out_stream_begin(os, c, m->out_compressor, m->out_chunk_len, m->out_max_compressed_len, out0.data, out0.data_cap, WS_CODEC));
     const uint64_t L = (uint64_t)m->out_chunk_len;
@@ -1815,6 +1846,7 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         mark(4);
         // the merged stream of this piece goes behind the unconsumed tail of the previous one; UOUT + tail_len is file offset ubase_total
         if (k5_async && r >= 2) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_pool[EV_K5 + 1 + (r & 1)], 0));      // K5 of piece r - 2 has read this buffer
+        if (raw_out && to_host_stream && r >= 2) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_pool[EV_K5 + 1 + (r & 1)], 0));      // piece r - 2's bytes have left it
         B200C_TRY(ws_typed(c, (r & 1) ? WS_UOUT2 : WS_UOUT, tail_len + ulen_out + 64, &UOUT));
         if (r) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_pool[EV_INDEX], 0));          // IOUT of the previous piece has left
         B200C_TRY(ws_typed(c, WS_IOUT, ilen_out + 64, &IOUT));
@@ -1895,6 +1927,7 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
                 k5_last = EV_K5 + 1 + (r & 1);
             }
             B200C_TRY(arc);
+            if (raw_out) B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_K5 + 1 + (r & 1)], c->copy_out));      // the read-back of this UOUT buffer
             tail_len = avail - take; tail_ptr = UOUT + take;
         }
         ubase_total += ulen_out; ilen_total += ilen_out;
@@ -2011,7 +2044,8 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         if (out.data_cap < bound) { c->err = "output data buffer too small"; timing_end(c); return B200C_ETOOSMALL; }
         uint64_t* d_ooffs; B200C_TRY(ws_typed(c, WS_OOFFS, nchunks_out + 2, &d_ooffs));
         uint64_t out_len = 0; uint32_t digest = 0;
-        B200C_TRY(compress_stream_device(c, m->out_compressor, UOUT, ulen_out, m->out_chunk_len, m->out_max_compressed_len, out.data, bound, d_ooffs, &out_len, &digest, WS_CODEC));
+        if (raw_out) { B200C_TRY(raw_stream_device(c, UOUT, ulen_out, m->out_chunk_len, out.data, d_ooffs, &digest, WS_CODEC)); out_len = ulen_out; }
+        else B200C_TRY(compress_stream_device(c, m->out_compressor, UOUT, ulen_out, m->out_chunk_len, m->out_max_compressed_len, out.data, bound, d_ooffs, &out_len, &digest, WS_CODEC));
         RunStats rs; B200C_TRY(finish_common(rs));
         res->noutputs = 1;
         out.data_len = out_len; out.index_len = ilen_out; out.nchunks = nchunks_out; out.data_length = ulen_out; out.digest = digest;
@@ -2027,11 +2061,14 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         // ---- multi-file output: one pass per file over a compressed window (see k_find_cut) ----------------------------------------
         const int comp = m->out_compressor; const int stride = chunk_slot_stride(comp, (int)L);
         const uint64_t nch_total = (ulen_out + L - 1) / L;
-        uint8_t* slots; uint32_t *file_len, *seg_raw; uint64_t *woffs, *d_dposf, *d_iposf, *d_cut, *d_ooffs; uint8_t *IOUTF, *d_dout; RunStats* d_fstats;
-        B200C_TRY(ws_typed(c, WS_CODEC + 2, (nch_total + 2) * (uint64_t)stride, &slots));
-        B200C_TRY(ws_typed(c, WS_CODEC + 3, nch_total + 2, &file_len));
-        B200C_TRY(ws_typed(c, WS_CODEC + 4, nch_total + 2, &seg_raw));
-        B200C_TRY(ws_typed(c, WS_LCS0, nch_total + 4, &woffs));
+        uint64_t *woffs = nullptr, *d_dposf, *d_iposf, *d_cut, *d_ooffs; uint8_t* IOUTF; RunStats* d_fstats;
+        uint8_t* slots = nullptr; uint32_t *file_len = nullptr, *seg_raw = nullptr; uint8_t* d_dout = nullptr;      // (compressed output only)
+        if (!raw_out) {
+            B200C_TRY(ws_typed(c, WS_CODEC + 2, (nch_total + 2) * (uint64_t)stride, &slots));
+            B200C_TRY(ws_typed(c, WS_CODEC + 3, nch_total + 2, &file_len));
+            B200C_TRY(ws_typed(c, WS_CODEC + 4, nch_total + 2, &seg_raw));
+        }
+        if (!raw_out) B200C_TRY(ws_typed(c, WS_LCS0, nch_total + 4, &woffs));
         B200C_TRY(ws_typed(c, WS_LCS1, nparts + 2, &d_dposf));
         B200C_TRY(ws_typed(c, WS_LCS2, nparts + 2, &d_iposf));
         B200C_TRY(ws_typed(c, WS_LCS3, 64, &d_cut)); d_fstats = (RunStats*)(d_cut + 8);
@@ -2039,18 +2076,24 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         B200C_TRY(ws_typed(c, WS_LCS4, ilen_out + 64, &IOUTF));
         B200C_TRY(ws_typed(c, WS_OOFFS, nch_total + 4, &d_ooffs));
         const uint64_t file_bound = b200c_compress_bound(comp, ulen_out, (int)L);
-        B200C_TRY(ws_typed(c, WS_DOUT, file_bound + 64, &d_dout));
+        if (!raw_out) B200C_TRY(ws_typed(c, WS_DOUT, file_bound + 64, &d_dout));
         res->required_data_cap = res->required_index_cap = res->required_chunk_cap = 0;
         uint64_t jlo = 0, start_b = 0; int f = 0;
         // how much of the stream to compress before looking for the file boundary: the file holds max_sstable_bytes of COMPRESSED chunks, so the
         // window is that divided by the ratio seen so far (the inputs' own ratio for the first file, then the previous file's) plus 8 %; a window
         // that turns out too short is extended below (doubling), nothing is compressed twice
         double est_ratio = 0.5;
-        { uint64_t ci = 0, ui = 0; for (int i = 0; i < K; i++) { ci += m->inputs[i].data_len; ui += m->inputs[i].data_length; } if (ui) est_ratio = std::min(1.0, std::max(0.05, (double)ci / (double)ui)); }
+        if (!raw_out) { uint64_t ci = 0, ui = 0; for (int i = 0; i < K; i++) { ci += m->inputs[i].data_len; ui += m->inputs[i].data_length; } if (ui) est_ratio = std::min(1.0, std::max(0.05, (double)ci / (double)ui)); }
         while (jlo < nparts && start_b < ulen_out) {
             B200C_TRY(check_cancel());
             const uint64_t remaining = ulen_out - start_b, rem_chunks = (remaining + L - 1) / L;
-            uint64_t want = std::max<uint64_t>(64, (uint64_t)((double)m->max_sstable_bytes / est_ratio * 1.08) / L + 8), done = 0, jhi = nparts, status = 2;
+            uint64_t want = 0, done = 0, jhi = nparts, status = raw_out ? 0 : 2;
+            if (raw_out) {                                   // the exact position decides (k_find_cut_raw): nothing to compress first
+                B200C_LAUNCH(c, k_find_cut_raw, 1, 1, 0, d_dpos, jlo, nparts, start_b, m->max_sstable_bytes, d_cut);
+                B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_cut, 8, cudaMemcpyDeviceToHost, st));
+                B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
+                jhi = h[0];
+            } else want = std::max<uint64_t>(64, (uint64_t)((double)m->max_sstable_bytes / est_ratio * 1.08) / L + 8);
             while (status == 2) {
                 uint64_t W = std::min(rem_chunks, want);
                 if (W > done) B200C_TRY(compress_slots_device(c, comp, UOUT + start_b + done * L, std::min(remaining - done * L, (W - done) * (uint64_t)L), (int)L,
@@ -2069,10 +2112,13 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
             uint64_t end_b = ulen_out;
             if (jhi < nparts) { B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_dpos + jhi, 8, cudaMemcpyDeviceToHost, st)); B200C_CUDA_TRY(c, cudaStreamSynchronize(st)); end_b = h[0]; }
             const uint64_t flen = end_b - start_b, fchunks = (flen + L - 1) / L, nfull = flen / L, tail = flen % L;
-            if (tail && !(end_b == ulen_out && done == rem_chunks))      // the last chunk of the file is shorter than what the window compressed there
-                B200C_TRY(compress_slots_device(c, comp, UOUT + start_b + nfull * L, tail, (int)L, m->out_max_compressed_len, slots + nfull * stride, stride, file_len + nfull, seg_raw + nfull));
             uint64_t out_len = 0; uint32_t digest = 0;
-            B200C_TRY(pack_digest_device(c, slots, stride, file_len, seg_raw, fchunks, d_dout, file_bound, d_ooffs, &out_len, &digest, WS_CODEC));
+            if (raw_out) { B200C_TRY(raw_stream_device(c, UOUT + start_b, flen, (int)L, nullptr, d_ooffs, &digest, WS_CODEC)); out_len = flen; }
+            else {
+                if (tail && !(end_b == ulen_out && done == rem_chunks))      // the last chunk of the file is shorter than what the window compressed there
+                    B200C_TRY(compress_slots_device(c, comp, UOUT + start_b + nfull * L, tail, (int)L, m->out_max_compressed_len, slots + nfull * stride, stride, file_len + nfull, seg_raw + nfull));
+                B200C_TRY(pack_digest_device(c, slots, stride, file_len, seg_raw, fchunks, d_dout, file_bound, d_ooffs, &out_len, &digest, WS_CODEC));
+            }
             // Index.db of this file: positions relative to the file start
             const uint64_t cnt = jhi - jlo;
             B200C_LAUNCH(c, k_rel_pos, (unsigned)((cnt + 1 + 255) / 256), 256, 0, d_dpos, jlo, jhi, start_b, d_dposf);
@@ -2101,7 +2147,7 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
                     if (out_len > o.data_cap || filen > o.index_cap || fchunks > o.chunk_cap) { c->err = "output buffers too small"; rc = B200C_ETOOSMALL; }
                     else {
                         cudaMemcpyKind k = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-                        if (out_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(o.data, d_dout, out_len, k, st));
+                        if (out_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(o.data, raw_out ? UOUT + start_b : d_dout, out_len, k, st));
                         if (filen) B200C_CUDA_TRY(c, cudaMemcpyAsync(o.index, IOUTF, filen, k, st));
                         if (fchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(o.chunk_offsets, d_ooffs, fchunks * 8, k, st));
                         B200C_CUDA_TRY(c, cudaStreamSynchronize(st));

@@ -13,6 +13,8 @@ using namespace b200c;
 namespace b200c {
 
 enum { WSC_IN = 0, WSC_OUT, WSC_SLOTS, WSC_FILELEN, WSC_SEGRAW, WSC_OFFS, WSC_ACC, WSC_ERR, WSC_CHOFFS, WSC_SCAN0, WSC_SCAN1, WSC_SCAN2 };
+int raw_chunks_device(b200c_ctx* c, bool ingest, const RawArgs& a);
+static int raw_digest(b200c_ctx* c, const uint32_t* seg_raw, const uint64_t* ends, uint64_t nchunks, uint32_t* acc, uint32_t* digest);
 
 static void build_tables(DevTables* t) {
     for (uint32_t i = 0; i < 256; i++) {
@@ -30,6 +32,10 @@ static void build_tables(DevTables* t) {
     for (int j = 0; j < 4; j++)
         for (uint32_t b = 0; b < 256; b++) t->crc_adv128[j][b] = gf2_mulmod(b << (8 * j), x128);
     for (int l = 0; l < 32; l++) t->xp_lane[l] = xpow8n(4 * (32 - l));
+    uint32_t x512 = xpow8n(512);
+    for (int j = 0; j < 4; j++)
+        for (uint32_t b = 0; b < 256; b++) t->crc_adv512[j][b] = gf2_mulmod(b << (8 * j), x512);
+    for (int l = 0; l < 32; l++) t->xp_lane16[l] = xpow8n(16 * (31 - l));
 }
 
 template <typename TIn>
@@ -144,6 +150,7 @@ __global__ void __launch_bounds__(256) k_offs_add_base(const uint64_t* __restric
 int out_stream_begin(OutStream& o, b200c_ctx* c, int comp, int chunk_len, int max_clen, uint8_t* h_out, uint64_t h_cap, int ws_base) {
     o = OutStream();
     o.c = c; o.comp = comp; o.L = chunk_len; o.max_clen = max_clen; o.stride = chunk_slot_stride(comp, chunk_len); o.ws_base = ws_base;
+    o.raw = comp == COMP_UNCOMPRESSED;
     o.h_out = h_out; o.h_cap = h_out ? h_cap : 0;
     B200C_TRY(ws_typed(c, ws_base + WSC_CHOFFS, (size_t)OutStream::MAX_PIECES + 2, &o.bases));
     B200C_TRY(ws_typed(c, ws_base + WSC_ACC, 4, &o.acc));
@@ -176,6 +183,25 @@ int out_stream_append(OutStream& o, const uint8_t* d_in, uint64_t nbytes) {
     if (o.piece >= OutStream::MAX_PIECES) { c->err = "internal error: too many output pieces"; return B200C_ECUDA; }
     const uint64_t k = (nbytes + o.L - 1) / o.L, a = o.nchunks;
     if (a + k > 0x7fffffffull) { c->err = "too many chunks"; return B200C_EINVAL; }
+    if (o.raw) {
+        // uncompressed: the CRC.db entries (d_offs) and digest registers of the piece's chunks, and its bytes go to the host straight from the
+        // merged stream; the caller keeps that buffer unchanged until the copy has left (compact.cu)
+        const int s = o.piece;
+        B200C_TRY(ws_grow_keep(c, o.ws_base + WSC_SEGRAW, a + k + 2, a, &o.seg_raw));
+        B200C_TRY(ws_grow_keep(c, o.ws_base + WSC_OFFS, a + k + 2, a, &o.d_offs));
+        B200C_TRY(ws_grow_keep(c, o.ws_base + WSC_FILELEN, a + k + 2, a + 1, &o.ends));
+        RawArgs ra; memset(&ra, 0, sizeof(ra));
+        ra.src = d_in; ra.n = nbytes; ra.L = o.L; ra.chunk_end = k; ra.crc_out = o.d_offs + a; ra.seg_raw = o.seg_raw + a; ra.ends = o.ends + a; ra.ebase = o.ulen;
+        B200C_TRY(raw_chunks_device(c, false, ra));
+        B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[2 * s], c->stream));
+        if (o.ulen + nbytes > o.h_cap) o.fits = false;
+        if (o.fits) {
+            B200C_CUDA_TRY(c, cudaStreamWaitEvent(c->copy_out, c->ev_pool[2 * s], 0));
+            B200C_CUDA_TRY(c, cudaMemcpyAsync(o.h_out + o.ulen, d_in, nbytes, cudaMemcpyDeviceToHost, c->copy_out));
+        }
+        o.nchunks += k; o.ulen += nbytes; o.copied = o.ulen; o.piece++;
+        return B200C_OK;
+    }
     uint8_t* slots; uint64_t* rel; const int s = o.piece;
     B200C_TRY(ws_grow_keep(c, o.ws_base + WSC_FILELEN, a + k + 2, a, &o.file_len));
     B200C_TRY(ws_grow_keep(c, o.ws_base + WSC_SEGRAW, a + k + 2, a, &o.seg_raw));
@@ -202,6 +228,12 @@ int out_stream_finish(OutStream& o, uint64_t* out_len, uint32_t* digest, uint64_
     b200c_ctx* c = o.c;
     *out_len = 0; *digest = 0; *d_offs_out = nullptr;
     if (!o.nchunks) return B200C_OK;
+    if (o.raw) {
+        B200C_TRY(raw_digest(c, o.seg_raw, o.ends, o.nchunks, o.acc, digest));
+        B200C_CUDA_TRY(c, cudaStreamSynchronize(c->copy_out));
+        *out_len = o.ulen; *d_offs_out = o.d_offs;
+        return B200C_OK;
+    }
     uint32_t* h32 = (uint32_t*)((uint64_t*)c->h_pinned + 1024 + OutStream::MAX_PIECES + 1);
     B200C_LAUNCH(c, k_digest, (unsigned)((o.nchunks + 255) / 256), 256, 0, c->d_tables, o.seg_raw, o.d_offs, o.nchunks, o.acc);
     B200C_LAUNCH(c, k_digest_final, 1, 1, 0, c->d_tables, o.d_offs, o.nchunks, o.acc);
@@ -288,6 +320,40 @@ int decompress_multi_device(b200c_ctx* c, K1Seg* segs, int nseg, int verify, Chu
     B200C_CUDA_TRY(c, cudaMemsetAsync(next, 0, sizeof(*next), c->stream));
     B200C_LAUNCH(c, k_decompress_multi_thr, k1_grid(c, total), K1_THREADS, c->k1_smem, c->d_tables, d, nseg, total, verify, d_err, next);
     return B200C_OK;
+}
+
+// uncompressed streams: chunks [a.chunk0, a.chunk_end), one block per chunk, eight blocks per SM looping over them
+int raw_chunks_device(b200c_ctx* c, bool ingest, const RawArgs& a) {
+    if (a.chunk_end <= a.chunk0) return B200C_OK;
+    const unsigned grid = (unsigned)std::min<uint64_t>(a.chunk_end - a.chunk0, (uint64_t)c->nsm * 8);
+    if (ingest) B200C_LAUNCH(c, k_raw_ingest, grid, RAW_THREADS, 0, c->d_tables, a);
+    else B200C_LAUNCH(c, k_raw_checksum, grid, RAW_THREADS, 0, c->d_tables, a);
+    return B200C_OK;
+}
+static int raw_digest(b200c_ctx* c, const uint32_t* seg_raw, const uint64_t* ends, uint64_t nchunks, uint32_t* acc, uint32_t* digest) {
+    B200C_LAUNCH(c, k_digest, (unsigned)((nchunks + 255) / 256), 256, 0, c->d_tables, seg_raw, ends, nchunks, acc);
+    B200C_LAUNCH(c, k_digest_final, 1, 1, 0, c->d_tables, ends, nchunks, acc);
+    uint32_t* h32 = (uint32_t*)c->h_pinned;
+    B200C_CUDA_TRY(c, cudaMemcpyAsync(h32, acc + 1, 4, cudaMemcpyDeviceToHost, c->stream));
+    B200C_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    *digest = h32[0];
+    return B200C_OK;
+}
+// ChecksummedSequentialWriter over a resident stream: d_out (optional) receives the bytes, d_crc[0..nchunks) the CRC.db entries, *digest
+// Digest.crc32 of the bytes alone
+int raw_stream_device(b200c_ctx* c, const uint8_t* d_in, uint64_t n, int chunk_len, uint8_t* d_out, uint64_t* d_crc, uint32_t* digest, int ws_base) {
+    const uint64_t nchunks = (n + chunk_len - 1) / chunk_len;
+    *digest = 0;
+    if (!nchunks) return B200C_OK;
+    uint32_t *seg_raw, *acc; uint64_t* ends;
+    B200C_TRY(ws_typed(c, ws_base + WSC_SEGRAW, nchunks + 1, &seg_raw));
+    B200C_TRY(ws_typed(c, ws_base + WSC_SCAN1, nchunks + 2, &ends));
+    B200C_TRY(ws_typed(c, ws_base + WSC_ACC, 4, &acc));
+    B200C_CUDA_TRY(c, cudaMemsetAsync(acc, 0, 16, c->stream));
+    RawArgs a; memset(&a, 0, sizeof(a));
+    a.src = d_in; a.dst = d_out; a.n = n; a.L = chunk_len; a.chunk_end = nchunks; a.crc_out = d_crc; a.seg_raw = seg_raw; a.ends = ends;
+    B200C_TRY(raw_chunks_device(c, false, a));
+    return raw_digest(c, seg_raw, ends, nchunks, acc, digest);
 }
 
 } // namespace b200c
@@ -387,6 +453,7 @@ int b200c_last_stage_ms(b200c_ctx* c, double* out, int n) {
 
 uint64_t b200c_chunk_count(uint64_t n, int chunk_len) { return chunk_len > 0 ? (n + chunk_len - 1) / chunk_len : 0; }
 uint64_t b200c_compress_bound(int comp, uint64_t n, int chunk_len) {
+    if (comp == COMP_UNCOMPRESSED) return n;             // Data.db is the stream itself
     uint64_t nch = b200c_chunk_count(n, chunk_len);
     int m = chunk_max_compressed(comp, chunk_len); if (m < chunk_len) m = chunk_len;
     return nch * ((uint64_t)m + 4) + 64;
@@ -395,7 +462,7 @@ int b200c_initial_compressed_buffer_length(int comp, int chunk_len) { return chu
 
 static int check_codec_args(b200c_ctx* c, int comp, int chunk_len) {
     if (!c) return B200C_EINVAL;
-    if (comp != COMP_LZ4 && !comp_is_snappy(comp) && comp != COMP_NONE) { c->err = "unknown compressor"; return B200C_EINVAL; }
+    if (comp != COMP_LZ4 && !comp_is_snappy(comp) && comp != COMP_NONE && comp != COMP_UNCOMPRESSED) { c->err = "unknown compressor"; return B200C_EINVAL; }
     if (chunk_len <= 0 || chunk_len > 65536 || (chunk_len & (chunk_len - 1))) { c->err = "chunk_len must be a power of two <= 64 KiB"; return B200C_EUNSUPPORTED; }
     return B200C_OK;
 }
@@ -415,6 +482,22 @@ int b200c_compress_chunks(b200c_ctx* c, int comp, const uint8_t* in, uint64_t n,
     }
     if (dev && chunk_offsets) d_offs = chunk_offsets;     // caller provides nchunks+1 entries on the device
     else B200C_TRY(ws_typed(c, WSC_OFFS, nchunks + 1, &d_offs));
+    if (comp == COMP_UNCOMPRESSED) {
+        // ChecksummedSequentialWriter: Data.db = the stream, chunk_offsets[0..nchunks) = the CRC.db entries, digest over the bytes alone
+        if (out_cap < n) { *out_len = n; c->err = "output buffer too small"; return B200C_ETOOSMALL; }
+        timing_begin(c);
+        int rc = raw_stream_device(c, d_in, n, chunk_len, dev ? d_out : nullptr, d_offs, digest, 0);
+        int rc2 = timing_end(c);
+        if (rc != B200C_OK) return rc;
+        if (rc2 != B200C_OK) return rc2;
+        *out_len = n;
+        if (!dev) {
+            if (n) B200C_CUDA_TRY(c, cudaMemcpyAsync(out, d_in, n, cudaMemcpyDeviceToHost, c->stream));
+            if (chunk_offsets && nchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(chunk_offsets, d_offs, nchunks * 8, cudaMemcpyDeviceToHost, c->stream));
+            B200C_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+        }
+        return B200C_OK;
+    }
     timing_begin(c);
     int rc = compress_stream_device(c, comp, d_in, n, chunk_len, max_clen, d_out, out_cap, d_offs, out_len, digest, 0);
     int rc2 = timing_end(c);
@@ -433,8 +516,44 @@ int b200c_decompress_chunks(b200c_ctx* c, int comp, const uint8_t* data, uint64_
     B200C_TRY(check_codec_args(c, comp, chunk_len));
     if ((!data && data_len) || (!chunk_offsets && nchunks) || (!out && data_length)) { c->err = "null argument"; return B200C_EINVAL; }
     if (nchunks != b200c_chunk_count(data_length, chunk_len)) { c->err = "chunk count does not match data_length"; return B200C_EINVAL; }
+    if (comp == COMP_UNCOMPRESSED && data_len != data_length) { c->err = "uncompressed Data.db: data_length must equal data_len"; return B200C_EINVAL; }
     cudaSetDevice(c->device);
     const bool dev = flags & B200C_FLAG_DEVICE_PTRS;
+    if (comp == COMP_UNCOMPRESSED) {
+        // every chunk checked against its CRC.db entry (chunk_offsets) and copied out; host buffers are verified where they were staged
+        const uint8_t* d_data = data; const uint64_t* d_crc = chunk_offsets;
+        if (!dev) {
+            uint8_t* p; B200C_TRY(ws_typed(c, WSC_IN, data_len + 64, &p));
+            if (data_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(p, data, data_len, cudaMemcpyHostToDevice, c->stream));
+            d_data = p;
+            uint64_t* po; B200C_TRY(ws_typed(c, WSC_CHOFFS, nchunks + 1, &po));
+            if (nchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(po, chunk_offsets, nchunks * 8, cudaMemcpyHostToDevice, c->stream));
+            d_crc = po;
+        }
+        ChunkErr* d_err; B200C_TRY(ws_typed(c, WSC_ERR, 1, &d_err));
+        B200C_CUDA_TRY(c, cudaMemsetAsync(d_err, 0xFF, sizeof(ChunkErr), c->stream));
+        RawArgs a; memset(&a, 0, sizeof(a));
+        a.src = d_data; a.dst = dev ? out : nullptr; a.n = data_len; a.L = chunk_len; a.chunk_end = nchunks; a.crc_exp = verify_crc ? d_crc : nullptr; a.err = d_err;
+        timing_begin(c);
+        int rc = raw_chunks_device(c, true, a);
+        int rc2 = timing_end(c);
+        if (rc != B200C_OK) return rc;
+        if (rc2 != B200C_OK) return rc2;
+        ChunkErr* h = (ChunkErr*)c->h_pinned;
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_err, sizeof(ChunkErr), cudaMemcpyDeviceToHost, c->stream));
+        B200C_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+        if (h->first_bad != ~0ull) {
+            const uint64_t chunk = (h->first_bad >> 8) & 0xFFFFFFFFFFull;
+            if (where) { where->input = 0; where->kind = 1; where->chunk = chunk; where->offset = chunk * (uint64_t)chunk_len; }
+            c->err = "chunk CRC mismatch at chunk " + std::to_string(chunk);
+            return B200C_ECORRUPT;
+        }
+        if (!dev && data_len) {
+            B200C_CUDA_TRY(c, cudaMemcpyAsync(out, d_data, data_len, cudaMemcpyDeviceToHost, c->stream));
+            B200C_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+        }
+        return B200C_OK;
+    }
     const uint8_t* d_data = data; const uint64_t* d_offs = chunk_offsets; uint8_t* d_out = out;
     if (!dev) {
         uint8_t* p; B200C_TRY(ws_typed(c, WSC_IN, data_len + 64, &p));
@@ -469,6 +588,7 @@ int b200c_decompress_chunks(b200c_ctx* c, int comp, const uint8_t* data, uint64_
 // ICompressor.compress: one buffer in, compressor output (no CRC) out.
 int b200c_compress(b200c_ctx* c, int comp, const uint8_t* in, int n, uint8_t* out, int out_cap) {
     if (!c || n < 0 || !out) return B200C_EINVAL;
+    if (comp == COMP_UNCOMPRESSED) { c->err = "compression disabled is not an ICompressor"; return B200C_EINVAL; }
     if (n > 65536) { c->err = "single-buffer compress is limited to 64 KiB"; return B200C_EUNSUPPORTED; }
     int chunk_len = 1; while (chunk_len < n) chunk_len <<= 1;
     if (n == 0) {   // degenerate: LZ4 of nothing = length prefix + one empty-literal token; Snappy = varint 0
@@ -489,6 +609,7 @@ int b200c_compress(b200c_ctx* c, int comp, const uint8_t* in, int n, uint8_t* ou
 // ICompressor.uncompress: compressor output in, plain bytes out; returns the decoded length.
 int b200c_uncompress(b200c_ctx* c, int comp, const uint8_t* in, int n, uint8_t* out, int out_cap) {
     if (!c || !in || n <= 0 || out_cap < 0) return B200C_EINVAL;
+    if (comp == COMP_UNCOMPRESSED) { c->err = "compression disabled is not an ICompressor"; return B200C_EINVAL; }
     int ulen;
     if (comp == COMP_LZ4) { if (n < 4) { c->err = "truncated"; return B200C_ECORRUPT; } ulen = (int)((uint32_t)in[0] | ((uint32_t)in[1] << 8) | ((uint32_t)in[2] << 16) | ((uint32_t)in[3] << 24)); }
     else if (comp_is_snappy(comp)) { uint32_t v = 0; int sh = 0, i = 0; bool ok = false; for (; i < n && i < 5; i++) { v |= (uint32_t)(in[i] & 0x7f) << sh; if (!(in[i] & 0x80)) { ok = true; break; } sh += 7; } if (!ok) { c->err = "bad varint"; return B200C_ECORRUPT; } ulen = (int)v; }

@@ -114,6 +114,7 @@ struct OutStream {
     uint32_t *file_len = nullptr, *seg_raw = nullptr, *acc = nullptr; uint64_t *d_offs = nullptr, *bases = nullptr;
     uint8_t* img[2] = {nullptr, nullptr}; uint64_t img_cap[2] = {0, 0};
     uint64_t nchunks = 0, ulen = 0, copied = 0; int piece = 0; bool fits = true;
+    bool raw = false; uint64_t* ends = nullptr;              // uncompressed output: d_offs holds the CRC.db entries, ends the chunk ends (digest)
 };
 int out_stream_begin(OutStream& o, b200c_ctx* c, int comp, int chunk_len, int max_clen, uint8_t* h_out, uint64_t h_cap, int ws_base);
 int out_stream_append(OutStream& o, const uint8_t* d_in, uint64_t nbytes);

@@ -13,7 +13,7 @@ import ctypes as C, time
 import numpy as np
 from .. import native
 from ..io import sstable as sst
-from ..io.compress import CompressionMetadata, COMPRESSOR_IDS, COMPRESSOR_NAMES
+from ..io.compress import CompressionMetadata, ChecksumMetadata, COMPRESSOR_IDS, COMPRESSOR_NAMES
 
 INT64_MIN, INT64_MAX = -(1 << 63), (1 << 63) - 1
 
@@ -37,8 +37,9 @@ class OutputSSTable:
         self.partitions = partitions; self.rows = rows
         self.filter = self.summary = self.first_key = self.last_key = None; self.stats = None
     def components(self):
-        c = {"Data.db": self.data, "Index.db": self.index, "CompressionInfo.db": self.compression.serialize(),
-             "Digest.crc32": str(self.digest).encode()}
+        # compression disabled: CRC.db instead of CompressionInfo.db (DataComponent.buildWriter, S/io/sstable/format/DataComponent.java:43-60)
+        meta = "CRC.db" if isinstance(self.compression, ChecksumMetadata) else "CompressionInfo.db"
+        c = {"Data.db": self.data, "Index.db": self.index, meta: self.compression.serialize(), "Digest.crc32": str(self.digest).encode()}
         if self.filter is not None: c["Filter.db"] = self.filter
         if self.summary is not None: c["Summary.db"] = self.summary
         return c
@@ -69,7 +70,10 @@ class CompactionTask:
                  max_sstable_bytes=0, token_range=(INT64_MIN, INT64_MAX), bloom=None, min_index_interval=128, with_metadata=False):
         self.inputs = list(inputs); self.controller = controller
         c0 = self.inputs[0].compression
-        self.compression = compression or CompressionMetadata(c0.compressor_name, c0.chunk_length, c0.max_compressed_length, 0, [])
+        if compression is None:
+            compression = ChecksumMetadata(c0.chunk_length, 0, []) if isinstance(c0, ChecksumMetadata) else \
+                          CompressionMetadata(c0.compressor_name, c0.chunk_length, c0.max_compressed_length, 0, [])
+        self.compression = compression
         self.column_index_size = column_index_size; self.max_sstable_bytes = max_sstable_bytes; self.token_range = token_range
         # with_metadata: also produce Filter.db, Summary.db, first/last key and the Statistics.db side band (SURVEY §8 f1). bloom = (hash count,
         # 64-bit words) as FilterFactory would size the filter (io.sstable.bloom_geometry(estimated keys, fp chance)); None = 0.01 over the input keys
@@ -148,15 +152,8 @@ class CompactionTask:
         self.out_columns = out_cols
         return m
 
-    def execute(self, engine, max_outputs=None):
-        """Runs the compaction through `engine(manifest_ptr, result_ptr) -> rc` and returns a CompactionResult."""
-        m = self.build_manifest()
-        total_in = sum(i.compression.data_length for i in self.inputs)
-        nout = max_outputs or (1 if not self.max_sstable_bytes else max(2, int(2 * total_in // max(self.max_sstable_bytes, 1)) + 2))
-        cl = self.compression.chunk_length
-        data_cap = native.lib().b200c_compress_bound(self.compression.compressor_id, total_in + 1024, cl) if engine.needs_lib_bound else total_in * 2 + (1 << 20)
-        index_cap = sum(len(i.index) for i in self.inputs) * 2 + (1 << 16)
-        chunk_cap = total_in // cl + 16
+    def _result(self, m, nout, data_cap, index_cap, chunk_cap):
+        """a b200c_result over `nout` output slots with buffers of the given capacities"""
         res = native.Result(); outs = (native.Output * nout)(); bufs = []; extra = []
         for o in outs:
             d = np.empty(data_cap, dtype=np.uint8); ix = np.empty(index_cap, dtype=np.uint8); co = np.zeros(chunk_cap, dtype=np.uint64)
@@ -168,14 +165,36 @@ class CompactionTask:
                 o.key_buf, o.key_cap, o.filter, o.filter_cap, o.summary, o.summary_cap = kb.ctypes.data, len(kb), fl.ctypes.data, len(fl), sm.ctypes.data, len(sm)
                 o.stats = C.pointer(st)
         res.noutputs_cap = nout; res.outputs = outs
-        t0 = time.perf_counter()
-        engine(m, res)
+        return res, outs, bufs, extra
+
+    def execute(self, engine, max_outputs=None):
+        """Runs the compaction through `engine(manifest_ptr, result_ptr) -> rc` and returns a CompactionResult."""
+        m = self.build_manifest()
+        total_in = sum(i.compression.data_length for i in self.inputs)
+        nout = max_outputs or (1 if not self.max_sstable_bytes else max(2, int(2 * total_in // max(self.max_sstable_bytes, 1)) + 2))
+        cl = self.compression.chunk_length
+        data_cap = native.lib().b200c_compress_bound(self.compression.compressor_id, total_in + 1024, cl) if engine.needs_lib_bound else total_in * 2 + (1 << 20)
+        index_cap = sum(len(i.index) for i in self.inputs) * 2 + (1 << 16)
+        chunk_cap = total_in // cl + 16
+        # the merged stream can be longer than the inputs' streams (every row's deltas are re-encoded against the output header's minima,
+        # which may lie far below an input's own): a call that finds the buffers too small reports what it needs and runs once more
+        for attempt in (0, 1):
+            res, outs, bufs, extra = self._result(m, nout, data_cap, index_cap, chunk_cap)
+            t0 = time.perf_counter()
+            try:
+                engine(m, res)
+                break
+            except native.B200CError as e:
+                if e.code != native.ETOOSMALL or attempt: raise
+                data_cap = max(data_cap, int(res.required_data_cap)); index_cap = max(index_cap, int(res.required_index_cap))
+                chunk_cap = max(chunk_cap, int(res.required_chunk_cap))
         wall = time.perf_counter() - t0
         r = CompactionResult()
         for k in range(res.noutputs):
             o = outs[k]; d, ix, co = bufs[k]
-            meta = CompressionMetadata(self.compression.compressor_name, cl, self.compression.max_compressed_length, int(o.data_length),
-                                       [int(x) for x in co[:o.nchunks]], self.compression.options)
+            if isinstance(self.compression, ChecksumMetadata): meta = ChecksumMetadata(cl, int(o.data_length), [int(x) for x in co[:o.nchunks]])
+            else: meta = CompressionMetadata(self.compression.compressor_name, cl, self.compression.max_compressed_length, int(o.data_length),
+                                             [int(x) for x in co[:o.nchunks]], self.compression.options)
             out = OutputSSTable(d[:o.data_len].tobytes(), ix[:o.index_len].tobytes(), meta, int(o.digest), int(o.partitions), int(o.rows))
             if self.with_metadata:
                 kb, fl, sm, st = extra[k]

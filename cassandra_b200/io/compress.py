@@ -4,6 +4,8 @@ ICompressor (S/io/compress/ICompressor.java:28-86): initialCompressedBufferLengt
 created by `create(options)` (S/schema/CompressionParams.java:266-283). The persisted class simple name stays
 `LZ4Compressor` / `SnappyCompressor` so stock nodes can read the files (S/io/compress/CompressionMetadata.java:379).
 CompressionMetadata: CompressionInfo.db reader/writer (S/io/compress/CompressionMetadata.java:113-160,375-431).
+ChecksumMetadata: CRC.db, which stands in for CompressionInfo.db when a table's compression is disabled
+(ChecksummedSequentialWriter, S/io/util/ChecksummedSequentialWriter.java).
 """
 import struct
 from .. import native
@@ -48,7 +50,15 @@ class SnappyCompressor(ICompressor):
     @classmethod
     def create(cls, ctx, options=None): return cls(ctx)
 
-COMPRESSOR_IDS = {"LZ4Compressor": native.COMP_LZ4, "SnappyCompressor": native.COMP_SNAPPY}
+class NoopCompressor(ICompressor):
+    """S/io/compress/NoopCompressor.java — the compressed format (CompressionInfo.db, inline CRCs) with a copy as its codec.
+    CompressionParams.NOOP uses 4 KiB chunks."""
+    compressor_id = native.COMP_NONE
+    simple_name = "NoopCompressor"
+    @classmethod
+    def create(cls, ctx, options=None): return cls(ctx)
+
+COMPRESSOR_IDS = {"LZ4Compressor": native.COMP_LZ4, "SnappyCompressor": native.COMP_SNAPPY, "NoopCompressor": native.COMP_NONE}
 COMPRESSOR_NAMES = {v: k for k, v in COMPRESSOR_IDS.items()}
 
 class CompressionMetadata:
@@ -96,3 +106,37 @@ def read_compressed(ctx, data_db: bytes, compression_info: bytes, verify_crc=Tru
     meta = CompressionMetadata.parse(compression_info)
     return ctx.decompress_chunks(meta.compressor_id, data_db, meta.chunk_offsets, meta.data_length, meta.chunk_length,
                                  meta.max_compressed_length, verify_crc)
+
+class ChecksumMetadata:
+    """CRC.db of an sstable written with compression disabled: BE i32 chunk size, then one BE i32 CRC32 per chunk of Data.db
+    (ChecksumWriter.writeChunkSize / appendDirect, S/io/util/ChecksumWriter.java:48-89). It takes CompressionMetadata's place in the
+    manifest: compressor id B200C_COMP_UNCOMPRESSED, the chunk table holds the CRCs, data_length is the length of Data.db."""
+    compressor_id = native.COMP_UNCOMPRESSED
+    compressor_name = None
+    max_compressed_length = native.INT32_MAX
+    DEFAULT_CHUNK_LENGTH = 65536            # SequentialWriterOption's default buffer size (S/io/util/SequentialWriterOption.java:107)
+    def __init__(self, chunk_length, data_length, crcs):
+        self.chunk_length = chunk_length; self.data_length = data_length; self.chunk_offsets = list(crcs); self.options = {}
+    @property
+    def crcs(self): return self.chunk_offsets
+    @classmethod
+    def parse(cls, b: bytes, data_length: int):
+        (cl,) = struct.unpack_from(">i", b, 0)
+        n = (len(b) - 4) // 4
+        return cls(cl, data_length, [x for x in struct.unpack_from(">%dI" % n, b, 4)])
+    def serialize(self) -> bytes:
+        return struct.pack(">i%dI" % len(self.chunk_offsets), self.chunk_length, *self.chunk_offsets)
+
+def uncompressed_params(chunk_length=ChecksumMetadata.DEFAULT_CHUNK_LENGTH):
+    """the output setting of a table with compression = {'enabled': false}"""
+    return ChecksumMetadata(chunk_length, 0, [])
+
+def write_uncompressed(ctx, stream: bytes, chunk_length=ChecksumMetadata.DEFAULT_CHUNK_LENGTH):
+    """ChecksummedSequentialWriter over a whole stream -> (Data.db bytes, CRC.db bytes, Digest.crc32 text)."""
+    data, crcs, digest = ctx.compress_chunks(native.COMP_UNCOMPRESSED, stream, chunk_length)
+    return data, ChecksumMetadata(chunk_length, len(stream), crcs).serialize(), str(digest)
+
+def read_uncompressed(ctx, data_db: bytes, crc_db: bytes, verify_crc=True) -> bytes:
+    """Data.db of an uncompressed sstable, every chunk checked against CRC.db -> the stream."""
+    meta = ChecksumMetadata.parse(crc_db, len(data_db))
+    return ctx.decompress_chunks(native.COMP_UNCOMPRESSED, data_db, meta.crcs, len(data_db), meta.chunk_length, native.INT32_MAX, verify_crc)

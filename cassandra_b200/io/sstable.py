@@ -8,7 +8,7 @@ Mirrors what the Java shim gets for free from SSTableReader (`sstable.header`, `
 """
 import os, struct
 from .. import native
-from .compress import CompressionMetadata
+from .compress import CompressionMetadata, ChecksumMetadata
 
 TIMESTAMP_EPOCH = 1442880000000000      # EncodingStats.TIMESTAMP_EPOCH (2015-09-22T00:00Z in µs), EncodingStats.java:47-64
 DELETION_TIME_EPOCH = 1442880000
@@ -194,7 +194,10 @@ class SSTable:
         """base_path: '<dir>/oa-1-big-' (descriptor prefix)."""
         rd = lambda c: open(base_path + c, "rb").read()
         st = parse_statistics(rd("Statistics.db"))
-        t = cls(rd("Data.db"), rd("Index.db"), CompressionMetadata.parse(rd("CompressionInfo.db")), st["header_stats"],
+        data = rd("Data.db")
+        # compression disabled: CRC.db stands in for CompressionInfo.db (ChecksummedSequentialWriter)
+        meta = CompressionMetadata.parse(rd("CompressionInfo.db")) if os.path.exists(base_path + "CompressionInfo.db") else ChecksumMetadata.parse(rd("CRC.db"), len(data))
+        t = cls(data, rd("Index.db"), meta, st["header_stats"],
                    (st["min_timestamp"], st["min_local_deletion_time"], st["min_ttl"]), st["clustering_types"],
                    st["regular_columns"], st["static_columns"], st["key_type"], generation=generation)
         if os.path.exists(base_path + "Summary.db"): t.summary_positions = parse_summary_positions(rd("Summary.db"))
@@ -230,8 +233,9 @@ def index_summary_positions(index: bytes, interval: int = 128):
     return np.asarray(out, dtype=np.uint64)
 
 def write_components(base_path: str, data: bytes, index: bytes, compression: CompressionMetadata, digest: int):
-    """Writes the components the engine produces (Data, Index, CompressionInfo, Digest). Statistics/Filter/Summary are
+    """Writes the components the engine produces (Data, Index, CompressionInfo or CRC.db, Digest). Statistics/Filter/Summary are
     SURVEY §8f 'next' rows and stay with the Java writer for now."""
-    for comp, payload in (("Data.db", data), ("Index.db", index), ("CompressionInfo.db", compression.serialize()),
+    meta = "CRC.db" if isinstance(compression, ChecksumMetadata) else "CompressionInfo.db"
+    for comp, payload in (("Data.db", data), ("Index.db", index), (meta, compression.serialize()),
                           ("Digest.crc32", str(digest).encode())):
         with open(base_path + comp, "wb") as f: f.write(payload)

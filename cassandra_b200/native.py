@@ -6,6 +6,7 @@ LIB_PATH = os.path.join(_HERE, "libb200compact.so")
 
 OK, EINVAL, ECUDA, ECORRUPT, ECANCELLED, EUNSUPPORTED, ENOMEM, ETOOSMALL = 0, -1, -2, -3, -4, -5, -6, -7
 COMP_NONE, COMP_LZ4, COMP_SNAPPY, COMP_SNAPPY15 = 0, 1, 2, 3
+COMP_UNCOMPRESSED = 4                 # compression disabled: Data.db + CRC.db (include/b200c.h)
 FLAG_DEVICE_PTRS = 1
 INT32_MAX = 0x7FFFFFFF
 MAX_CLUSTERING, MAX_COLUMNS, MAX_INPUTS, MAX_STATIC_COLUMNS = 8, 64, 64, 16

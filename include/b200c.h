@@ -49,6 +49,29 @@ enum {
  * written by Google snappy >= 1.2.0 (hash table of at most 2^15 entries: different, equally valid bytes; what newer snappy-java bundles, and the
  * generation tests/golden/snappy pins against the real library). Decompression is identical for both. */
 enum { B200C_COMP_NONE = 0, B200C_COMP_LZ4 = 1, B200C_COMP_SNAPPY = 2, B200C_COMP_SNAPPY15 = 3 };
+/* NONE is NoopCompressor (S/io/compress/NoopCompressor.java): the compressed format with a copy as its codec (CompressionInfo.db, inline
+ * CRCs; a chunk is never shorter than its data, so flushData's raw-storage rule never changes it).
+ * UNCOMPRESSED is a table with compression = {'enabled': false}: DataComponent.buildWriter (S/io/sstable/format/DataComponent.java:43-60)
+ * then writes Data.db through ChecksummedSequentialWriter (S/io/util/ChecksummedSequentialWriter.java). It is not an ICompressor:
+ * b200c_compress / b200c_uncompress refuse it with B200C_EINVAL. Same structs, no layout change — the fields mean:
+ *   data / data_len        the uncompressed Data.db itself; data_length must equal data_len (B200C_EINVAL otherwise). Index.db
+ *                          positions are positions in it.
+ *   chunk_len              CRC.db's chunk size (its leading BE i32): a power of two <= 64 KiB. Writers use 65536, the
+ *                          SequentialWriterOption default buffer (S/io/util/SequentialWriterOption.java:107).
+ *   chunk_offsets[i]       CRC.db's entry i zero-extended to 64 bits in native order: the CRC32 of Data.db bytes
+ *                          [i * chunk_len, min((i + 1) * chunk_len, data_len)). nchunks = ceil(data_len / chunk_len) (B200C_EINVAL
+ *                          otherwise): every chunk is full but the last, and a file whose length is a multiple of chunk_len has no
+ *                          empty trailing chunk (the buffer is flushed only when full and once at the end).
+ *   max_compressed_len     ignored.
+ * Inputs: every chunk is verified against its entry (B200C_ECORRUPT, kind 1, chunk i, offset i * chunk_len). CRC.db is required.
+ * Outputs (out_compressor): data receives Data.db (data_len == data_length), chunk_offsets the CRC.db entries (chunk_cap counts them),
+ * digest is the CRC32 of Data.db alone (no per-chunk CRCs mixed in). An LCS writer (max_sstable_bytes != 0) switches files before the
+ * first partition that starts more than max_sstable_bytes into the file: for an uncompressed writer getEstimatedOnDiskBytesWritten()
+ * is position(), which counts the bytes still buffered (S/io/util/SequentialWriter.java:304-312,342-345).
+ * Inputs of one call may mix every id here; the output's need not match any input's. b200c_compress_bound(UNCOMPRESSED, n, L) = n.
+ * b200c_compress_chunks(UNCOMPRESSED) is ChecksummedSequentialWriter (copy, CRC.db entries in chunk_offsets, digest);
+ * b200c_decompress_chunks(UNCOMPRESSED) checks every chunk against its entry (when verify_crc) and copies it out. */
+enum { B200C_COMP_UNCOMPRESSED = 4 };
 /* IPartitioner of the table (ValidationMetadata.partitioner, S/io/sstable/metadata/ValidationMetadata.java): decides the partition
  * order every input must already be in and the output is written in (DecoratedKey.compareTo, S/db/DecoratedKey.java:79-91).
  *   MURMUR3       S/dht/Murmur3Partitioner.java:256-296 — signed 64-bit token, ties by unsigned key bytes

@@ -21,7 +21,7 @@ public final class B200C
 
     // ---- return codes of b200c.h --------------------------------------------------------------------------------------------
     public static final int OK = 0, EINVAL = -1, ECUDA = -2, ECORRUPT = -3, ECANCELLED = -4, EUNSUPPORTED = -5, ENOMEM = -6, ETOOSMALL = -7;
-    public static final int COMP_NONE = 0, COMP_LZ4 = 1, COMP_SNAPPY = 2;
+    public static final int COMP_NONE = 0, COMP_LZ4 = 1, COMP_SNAPPY = 2, COMP_UNCOMPRESSED = 4;      // 4: compression disabled, Data.db + CRC.db
     public static final int PARTITIONER_MURMUR3 = 0, PARTITIONER_BYTE_ORDERED = 1;
     public static final int TYPE_BYTES = 0, TYPE_FIXED_SIGNED = 1, TYPE_FIXED_BYTES = 2, TYPE_VAR_SIGNED = 3, TYPE_TIMEUUID = 4, TYPE_COUNTER = 5;
     public static final int MAX_COMPLEX_COLUMNS = 8;       // multi-cell (map / set / list) columns per table, B200C_MAX_COMPLEX_COLUMNS

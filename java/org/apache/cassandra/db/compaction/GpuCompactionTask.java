@@ -94,7 +94,13 @@ public class GpuCompactionTask extends CompactionTask
         for (SSTableReader r : inputs)
         {
             if (!(r instanceof BigTableReader) || !r.descriptor.version.version.equals("oa")) return false;
-            if (!r.compression) return false;
+            if (!r.compression)
+            {
+                // compression disabled: Data.db + CRC.db (ChecksummedSequentialWriter); the engine verifies every chunk against CRC.db
+                int chunk = crcChunkSize(r);
+                if (chunk <= 0 || chunk > 65536 || (chunk & (chunk - 1)) != 0) return false;
+                continue;
+            }
             String comp = r.getCompressionMetadata().parameters.getSstableCompressor().getClass().getSimpleName();
             if (compressorId(comp) < 0 || r.getCompressionMetadata().chunkLength() > 65536) return false;
         }
@@ -105,7 +111,22 @@ public class GpuCompactionTask extends CompactionTask
     {
         if (simpleName.endsWith("LZ4Compressor")) return B200C.COMP_LZ4;
         if (simpleName.endsWith("SnappyCompressor")) return B200C.COMP_SNAPPY;
+        if (simpleName.equals("NoopCompressor")) return B200C.COMP_NONE;
         return -1;
+    }
+
+    /** CRC.db's leading BE i32 (ChecksumWriter.writeChunkSize), -1 when the file is missing or unreadable */
+    static int crcChunkSize(SSTableReader r)
+    {
+        File f = r.descriptor.fileFor(Components.CRC);
+        if (!f.exists()) return -1;
+        try (FileChannel ch = FileChannel.open(f.toPath(), StandardOpenOption.READ))
+        {
+            ByteBuffer b = ByteBuffer.allocate(4).order(ByteOrder.BIG_ENDIAN);
+            while (b.hasRemaining()) if (ch.read(b) < 0) return -1;
+            return b.getInt(0);
+        }
+        catch (IOException e) { return -1; }
     }
 
     /** comparison / layout class of a value type (b200c.h B200C_TYPE_*): -1 = outside the envelope */
@@ -166,24 +187,43 @@ public class GpuCompactionTask extends CompactionTask
         final MappedByteBuffer data, index;
         final ByteBuffer chunkOffsets, summaryPositions;
         final long nChunks, nSummary;
+        final int compressor, chunkLength, maxCompressedLength;
+        final long dataLength;                                      // uncompressed length
 
         Input(SSTableReader r) throws IOException
         {
             reader = r;
             data = map(r.descriptor.fileFor(Components.DATA));
             index = map(r.descriptor.fileFor(BigFormat.Components.PRIMARY_INDEX));
-            // CompressionInfo.db: UTF name | i32 nOpts | (UTF,UTF)* | i32 chunkLength | i32 maxCompressedLength | i64 dataLength | i32 n | i64 offset x n (BE)
-            CompressionMetadata cm = r.getCompressionMetadata();
-            ByteBuffer info = map(r.descriptor.fileFor(Components.COMPRESSION_INFO)).order(ByteOrder.BIG_ENDIAN);
-            int p = 2 + (info.getShort(0) & 0xFFFF);
-            int nOpts = info.getInt(p); p += 4;
-            for (int i = 0; i < 2 * nOpts; i++) p += 2 + (info.getShort(p) & 0xFFFF);
-            p += 4 + 4 + 8;
-            int n = info.getInt(p); p += 4;
-            nChunks = n;
-            chunkOffsets = B200C.struct(8 * Math.max(n, 1));
-            for (int i = 0; i < n; i++) chunkOffsets.putLong(8 * i, info.getLong(p + 8 * i));
-            assert cm.dataLength >= 0;
+            if (r.compression)
+            {
+                // CompressionInfo.db: UTF name | i32 nOpts | (UTF,UTF)* | i32 chunkLength | i32 maxCompressedLength | i64 dataLength | i32 n | i64 offset x n (BE)
+                CompressionMetadata cm = r.getCompressionMetadata();
+                ByteBuffer info = map(r.descriptor.fileFor(Components.COMPRESSION_INFO)).order(ByteOrder.BIG_ENDIAN);
+                int p = 2 + (info.getShort(0) & 0xFFFF);
+                int nOpts = info.getInt(p); p += 4;
+                for (int i = 0; i < 2 * nOpts; i++) p += 2 + (info.getShort(p) & 0xFFFF);
+                p += 4 + 4 + 8;
+                int n = info.getInt(p); p += 4;
+                nChunks = n;
+                chunkOffsets = B200C.struct(8 * Math.max(n, 1));
+                for (int i = 0; i < n; i++) chunkOffsets.putLong(8 * i, info.getLong(p + 8 * i));
+                assert cm.dataLength >= 0;
+                compressor = compressorId(cm.parameters.getSstableCompressor().getClass().getSimpleName());
+                chunkLength = cm.chunkLength(); maxCompressedLength = cm.maxCompressedLength(); dataLength = cm.dataLength;
+            }
+            else
+            {
+                // compression disabled. CRC.db: BE i32 chunk size | BE i32 CRC32 per chunk of Data.db; the chunk table carries the CRCs
+                // zero-extended in native order (include/b200c.h, B200C_COMP_UNCOMPRESSED)
+                ByteBuffer crc = map(r.descriptor.fileFor(Components.CRC)).order(ByteOrder.BIG_ENDIAN);
+                int n = (crc.capacity() - 4) / 4;
+                nChunks = n;
+                chunkOffsets = B200C.struct(8 * Math.max(n, 1));
+                for (int i = 0; i < n; i++) chunkOffsets.putLong(8 * i, crc.getInt(4 + 4 * i) & 0xFFFFFFFFL);
+                compressor = B200C.COMP_UNCOMPRESSED;
+                chunkLength = crc.getInt(0); maxCompressedLength = Integer.MAX_VALUE; dataLength = data.capacity();
+            }
             // Summary.db sample positions: already in memory for every open big-format reader (IndexSummary.getPosition :190-193)
             IndexSummary s = ((BigTableReader) r).getIndexSummary();
             nSummary = s.size();
@@ -240,13 +280,12 @@ public class GpuCompactionTask extends CompactionTask
                 for (int i = 0; i < inputs.size(); i++)
                 {
                     Input s = inputs.get(i); int o = i * SIZEOF_INPUT;
-                    CompressionMetadata cm = s.reader.getCompressionMetadata();
                     in.putLong(o + IN_DATA, B200C.address(s.data)).putLong(o + IN_DATA_LEN, s.data.capacity());
                     in.putLong(o + IN_INDEX, B200C.address(s.index)).putLong(o + IN_INDEX_LEN, s.index.capacity());
                     in.putLong(o + IN_CHUNK_OFFSETS, B200C.address(s.chunkOffsets)).putLong(o + IN_NCHUNKS, s.nChunks);
-                    in.putLong(o + IN_DATA_LENGTH, cm.dataLength);
-                    in.putInt(o + IN_COMPRESSOR, compressorId(cm.parameters.getSstableCompressor().getClass().getSimpleName()));
-                    in.putInt(o + IN_CHUNK_LEN, cm.chunkLength()).putInt(o + IN_MAX_COMPRESSED_LEN, cm.maxCompressedLength());
+                    in.putLong(o + IN_DATA_LENGTH, s.dataLength);
+                    in.putInt(o + IN_COMPRESSOR, s.compressor);
+                    in.putInt(o + IN_CHUNK_LEN, s.chunkLength).putInt(o + IN_MAX_COMPRESSED_LEN, s.maxCompressedLength);
                     List<ColumnMetadata> have = new ArrayList<>();
                     s.reader.header.columns().regulars.forEach(have::add);
                     in.putInt(o + IN_NCOLUMNS, have.size());
@@ -259,10 +298,14 @@ public class GpuCompactionTask extends CompactionTask
                     in.putLong(o + IN_HEADER_STATS, hs.minTimestamp).putLong(o + IN_HEADER_STATS + 8, hs.minLocalDeletionTime).putInt(o + IN_HEADER_STATS + 16, hs.minTTL);
                     in.putInt(o + IN_LEVEL, s.reader.getSSTableLevel());
                     in.putLong(o + IN_SUMMARY_POSITIONS, B200C.address(s.summaryPositions)).putLong(o + IN_NSUMMARY, s.nSummary);
-                    totalIn += cm.dataLength; totalIndex += s.index.capacity();
+                    totalIn += s.dataLength; totalIndex += s.index.capacity();
                 }
                 CompressionParams cp = table.params.compression;
-                int outComp = compressorId(cp.getSstableCompressor().getClass().getSimpleName());
+                // compression disabled (getSstableCompressor() is null): Data.db + CRC.db in the writer's 64 KiB buffer chunks
+                // (DataComponent.buildWriter, SequentialWriterOption's default buffer size)
+                final boolean compressed = cp.isEnabled();
+                int outComp = compressed ? compressorId(cp.getSstableCompressor().getClass().getSimpleName()) : B200C.COMP_UNCOMPRESSED;
+                int outChunk = compressed ? cp.chunkLength() : 65536, outMaxClen = compressed ? cp.maxCompressedLength() : Integer.MAX_VALUE;
                 ByteBuffer m = B200C.struct(SIZEOF_MANIFEST);
                 m.putInt(M_ABI_VERSION, B200C.ABI_VERSION).putInt(M_NINPUTS, inputs.size()).putLong(M_INPUTS, B200C.address(in));
                 m.putInt(M_NCLUSTERING, table.clusteringColumns().size());
@@ -278,7 +321,7 @@ public class GpuCompactionTask extends CompactionTask
                 for (int k = 0; k < outStatics.size(); k++)
                     m.putInt(M_STATIC_COLUMNS + 8 * k, columnClass(outStatics.get(k).type)).putInt(M_STATIC_COLUMNS + 8 * k + 4, Math.max(0, outStatics.get(k).type.valueLengthIfFixed()));
                 m.putLong(M_OUT_STATS, outStats.minTimestamp).putLong(M_OUT_STATS + 8, outStats.minLocalDeletionTime).putInt(M_OUT_STATS + 16, outStats.minTTL);
-                m.putInt(M_OUT_COMPRESSOR, outComp).putInt(M_OUT_CHUNK_LEN, cp.chunkLength()).putInt(M_OUT_MAX_COMPRESSED_LEN, cp.maxCompressedLength());
+                m.putInt(M_OUT_COMPRESSOR, outComp).putInt(M_OUT_CHUNK_LEN, outChunk).putInt(M_OUT_MAX_COMPRESSED_LEN, outMaxClen);
                 m.putInt(M_COLUMN_INDEX_SIZE, DatabaseDescriptor.getColumnIndexSize(BigFormat.getInstance().getDefaultColumnIndexSize()));
                 m.putLong(M_NOW_IN_SEC, nowInSec).putLong(M_GC_BEFORE, controller.gcBefore);
                 // purge evaluator: min timestamp over the live sstables / memtables that overlap the compaction (CompactionController.java:247-286).
@@ -298,40 +341,51 @@ public class GpuCompactionTask extends CompactionTask
                 m.putInt(M_MIN_INDEX_INTERVAL, table.params.minIndexInterval);
 
                 // ---- result + caller-provided output buffers ------------------------------------------------------------------------------------
-                long dataCap = B200C.compressBound(outComp, totalIn, cp.chunkLength());
-                ByteBuffer outData = ByteBuffer.allocateDirect(Math.toIntExact(Math.min(dataCap, Integer.MAX_VALUE - 8)));   // > 2 GiB outputs: use several buffers / Unsafe
-                ByteBuffer outIndex = ByteBuffer.allocateDirect(Math.toIntExact(totalIndex + (1 << 20)));
-                ByteBuffer outOffsets = B200C.struct(Math.toIntExact(8 * (totalIn / cp.chunkLength() + 16)));
+                // The merged stream can be longer than the inputs' streams (every row's deltas are re-encoded against the output header's minima,
+                // which may lie far below an input's own), so the first sizing is a guess: a call that returns ETOOSMALL has reported what it
+                // needs, and runs once more with buffers of that size.
+                long dataCap = B200C.compressBound(outComp, totalIn, outChunk), indexCap = totalIndex + (1 << 20), chunkCap = totalIn / outChunk + 16;
+                ByteBuffer outData, outIndex, outOffsets, out, res;
                 ByteBuffer keys = ByteBuffer.allocateDirect(2 * 65535);
                 ByteBuffer filter = B200C.struct(Math.toIntExact(8 + 8 * m.getLong(M_BLOOM_WORDS)));
                 ByteBuffer summary = ByteBuffer.allocateDirect(Math.toIntExact(totalIndex / 16 + (1 << 20)));
                 ByteBuffer stats = B200C.struct(SIZEOF_STATS);
-                ByteBuffer out = B200C.struct(SIZEOF_OUTPUT);
-                out.putLong(O_DATA, B200C.address(outData)).putLong(O_DATA_CAP, outData.capacity());
-                out.putLong(O_INDEX, B200C.address(outIndex)).putLong(O_INDEX_CAP, outIndex.capacity());
-                out.putLong(O_CHUNK_OFFSETS, B200C.address(outOffsets)).putLong(O_CHUNK_CAP, outOffsets.capacity() / 8);
-                out.putLong(O_KEY_BUF, B200C.address(keys)).putLong(O_KEY_CAP, keys.capacity());
-                out.putLong(O_FILTER, B200C.address(filter)).putLong(O_FILTER_CAP, filter.capacity());
-                out.putLong(O_SUMMARY, B200C.address(summary)).putLong(O_SUMMARY_CAP, summary.capacity());
-                out.putLong(O_STATS, B200C.address(stats));
-                ByteBuffer res = B200C.struct(SIZEOF_RESULT);
-                res.putInt(R_NOUTPUTS_CAP, 1).putLong(R_OUTPUTS, B200C.address(out));
-                B200C.hostRegister(B200C.address(outData), outData.capacity());
-
-                // ---- the call; progress and stop requests travel through poll / cancel from the CompactionInfo.Holder ------------------------------
                 GpuCompactionInfo info = new GpuCompactionInfo(this, ctx, totalIn);
-                CompactionManager.instance.active.beginCompaction(info);
                 int rc;
-                try
+                for (int attempt = 0; ; attempt++)
                 {
-                    if (!cfs.getCompactionStrategyManager().isActive())
-                        throw new CompactionInterruptedException(info.getCompactionInfo());
-                    rc = B200C.compact(ctx, B200C.address(m), B200C.address(res), 0);
-                }
-                finally
-                {
-                    CompactionManager.instance.active.finishCompaction(info);
-                    B200C.hostUnregister(B200C.address(outData));
+                    outData = ByteBuffer.allocateDirect(Math.toIntExact(Math.min(dataCap, Integer.MAX_VALUE - 8)));   // > 2 GiB outputs: use several buffers / Unsafe
+                    outIndex = ByteBuffer.allocateDirect(Math.toIntExact(indexCap));
+                    outOffsets = B200C.struct(Math.toIntExact(8 * chunkCap));
+                    out = B200C.struct(SIZEOF_OUTPUT);
+                    out.putLong(O_DATA, B200C.address(outData)).putLong(O_DATA_CAP, outData.capacity());
+                    out.putLong(O_INDEX, B200C.address(outIndex)).putLong(O_INDEX_CAP, outIndex.capacity());
+                    out.putLong(O_CHUNK_OFFSETS, B200C.address(outOffsets)).putLong(O_CHUNK_CAP, outOffsets.capacity() / 8);
+                    out.putLong(O_KEY_BUF, B200C.address(keys)).putLong(O_KEY_CAP, keys.capacity());
+                    out.putLong(O_FILTER, B200C.address(filter)).putLong(O_FILTER_CAP, filter.capacity());
+                    out.putLong(O_SUMMARY, B200C.address(summary)).putLong(O_SUMMARY_CAP, summary.capacity());
+                    out.putLong(O_STATS, B200C.address(stats));
+                    res = B200C.struct(SIZEOF_RESULT);
+                    res.putInt(R_NOUTPUTS_CAP, 1).putLong(R_OUTPUTS, B200C.address(out));
+                    B200C.hostRegister(B200C.address(outData), outData.capacity());
+
+                    // ---- the call; progress and stop requests travel through poll / cancel from the CompactionInfo.Holder ------------------------------
+                    CompactionManager.instance.active.beginCompaction(info);
+                    try
+                    {
+                        if (!cfs.getCompactionStrategyManager().isActive())
+                            throw new CompactionInterruptedException(info.getCompactionInfo());
+                        rc = B200C.compact(ctx, B200C.address(m), B200C.address(res), 0);
+                    }
+                    finally
+                    {
+                        CompactionManager.instance.active.finishCompaction(info);
+                        B200C.hostUnregister(B200C.address(outData));
+                    }
+                    if (rc != B200C.ETOOSMALL || attempt > 0) break;
+                    dataCap = Math.max(dataCap, res.getLong(R_REQUIRED_DATA_CAP));
+                    indexCap = Math.max(indexCap, res.getLong(R_REQUIRED_INDEX_CAP));
+                    chunkCap = Math.max(chunkCap, res.getLong(R_REQUIRED_CHUNK_CAP));
                 }
                 switch (rc)
                 {
@@ -351,18 +405,24 @@ public class GpuCompactionTask extends CompactionTask
                 if (out.getLong(O_PARTITIONS) > 0)
                 {
                     Descriptor d = cfs.newSSTableDescriptor(getDirectories().getWriteableLocationAsFile(cfs, null, out.getLong(O_DATA_LEN)));
-                    Set<Component> components = new java.util.HashSet<>(d.getFormat().allComponents());
+                    // exactly the components written below (+ TOC.txt): CompressionInfo.db or, with compression disabled, CRC.db
+                    Set<Component> components = new java.util.HashSet<>(java.util.Arrays.asList(Components.DATA, BigFormat.Components.PRIMARY_INDEX, Components.FILTER,
+                                                                                                 BigFormat.Components.SUMMARY, Components.DIGEST, Components.STATS, Components.TOC,
+                                                                                                 compressed ? Components.COMPRESSION_INFO : Components.CRC));
                     transaction.trackNew(new org.apache.cassandra.io.sstable.SSTable.Builder<>(d).setComponents(components).setTableMetadataRef(cfs.metadata).build(cfs));
                     write(d.fileFor(Components.DATA), outData, out.getLong(O_DATA_LEN));
                     write(d.fileFor(BigFormat.Components.PRIMARY_INDEX), outIndex, out.getLong(O_INDEX_LEN));
                     write(d.fileFor(Components.FILTER), filter, out.getLong(O_FILTER_LEN));
                     write(d.fileFor(BigFormat.Components.SUMMARY), summary, out.getLong(O_SUMMARY_LEN));
-                    writeCompressionInfo(d, cp, out, outOffsets);
+                    if (compressed) writeCompressionInfo(d, cp, out, outOffsets);
+                    else writeCrc(d, outChunk, out, outOffsets);
                     try (FileOutputStreamPlus o = new FileOutputStreamPlus(d.fileFor(Components.DIGEST)))
                     {
                         o.write(Long.toString(out.getInt(O_DIGEST) & 0xFFFFFFFFL).getBytes(java.nio.charset.StandardCharsets.UTF_8));
                     }
-                    writeStatistics(d, table, header, stats, keys, out, (double) out.getLong(O_DATA_LEN) / Math.max(1, out.getLong(O_DATA_LENGTH)), actuallyCompact, fp);
+                    double ratio = compressed ? (double) out.getLong(O_DATA_LEN) / Math.max(1, out.getLong(O_DATA_LENGTH))
+                                              : org.apache.cassandra.io.sstable.metadata.MetadataCollector.NO_COMPRESSION_RATIO;      // MetadataCollector.java:56,114
+                    writeStatistics(d, table, header, stats, keys, out, ratio, actuallyCompact, fp);
                     d.getFormat().getWriterFactory();                                            // TOC.txt
                     org.apache.cassandra.io.sstable.format.TOCComponent.appendTOC(d, components);
                     SSTableReader reader = SSTableReader.open(cfs, d, components, cfs.metadata);
@@ -407,6 +467,17 @@ public class GpuCompactionTask extends CompactionTask
             int n = Math.toIntExact(out.getLong(O_NCHUNKS));
             o.writeInt(n);
             for (int i = 0; i < n; i++) o.writeLong(offsets.getLong(8 * i));
+        }
+    }
+
+    /** CRC.db as ChecksumWriter writes it (S/io/util/ChecksumWriter.java:48-89): BE i32 chunk size, then the BE i32 CRC32 of every chunk */
+    private static void writeCrc(Descriptor d, int chunkLength, ByteBuffer out, ByteBuffer crcs) throws IOException
+    {
+        try (DataOutputStreamPlus o = new FileOutputStreamPlus(d.fileFor(Components.CRC)))
+        {
+            o.writeInt(chunkLength);
+            int n = Math.toIntExact(out.getLong(O_NCHUNKS));
+            for (int i = 0; i < n; i++) o.writeInt((int) crcs.getLong(8 * i));
         }
     }
 
