@@ -23,7 +23,6 @@
 #include <climits>
 #include <vector>
 #include <algorithm>
-#include <functional>
 #include <cmath>
 
 using namespace b200c;
@@ -51,7 +50,6 @@ static_assert(IW_PAD <= 64, "the Index.db workspace keeps 64 bytes behind every 
 #ifndef B200C_K1_BATCH_DEFAULT
 #define B200C_K1_BATCH_DEFAULT true
 #endif
-enum { MAX_RANGES = 16, EV_RANGE = 200, EV_INDEX = 220, EV_K5 = 230 };      // token-range pieces per call; slots of b200c_ctx::ev_pool
 #define NONE64 (~0ull)
 
 enum { WS_U = 16, WS_CD, WS_CO, WS_IDX, WS_PARAMS, WS_BBASE, WS_ISTART, WS_ICNT, WS_IEND, WS_IHIT, WS_IBAD, WS_ISCAN,
@@ -978,311 +976,409 @@ __global__ void __launch_bounds__(256) k_rel_pos(const uint64_t* __restrict__ dp
 
 } // namespace b200c
 
-// ---------------------------------------------------------------------------------------------------------------------------------
-extern "C" {
+// ---- b200c_compact, stage by stage ----------------------------------------------------------------------------------------------------
+// One CompactCall per call holds what the call was given, its plan (Index.db slices, token-range pieces, the chunks every piece needs)
+// and the device arrays one stage hands to the next. b200c_compact runs the stages in order; every return goes through the destructor.
+namespace {
 
-int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int flags) {
-    if (!c || !m || !res) return B200C_EINVAL;
-    auto t_start = std::chrono::steady_clock::now();
-    cudaSetDevice(c->device);
-    c->prog_stage.store(0); c->prog_scanned.store(0);
-    for (int i = 0; i < B200C_MAX_INPUTS; i++) c->prog_input_pos[i].store(0);
-    c->prog_seq.fetch_add(1);              // after the resets: figures read behind a new call_seq belong to this call
-    if (m->abi_version != B200C_ABI_VERSION || m->ninputs <= 0) { c->err = "bad manifest"; return B200C_EINVAL; }
-    if (m->partitioner != B200C_PARTITIONER_MURMUR3 && m->partitioner != B200C_PARTITIONER_BYTE_ORDERED) { c->err = "partitioner not supported (Murmur3Partitioner and ByteOrderedPartitioner are)"; return B200C_EUNSUPPORTED; }
-    if (m->partitioner == B200C_PARTITIONER_BYTE_ORDERED && (m->token_lo != INT64_MIN || m->token_hi != INT64_MAX || m->npurge_ranges)) { c->err = "ByteOrderedPartitioner: token sub-ranges are not expressible"; return B200C_EUNSUPPORTED; }
-    if (m->npurge_ranges < 0 || (m->npurge_ranges && (!m->purge_range_hi || !m->purge_range_max_ts))) { c->err = "purge table"; return B200C_EINVAL; }
-    for (int k = 1; k < m->npurge_ranges; k++) if (m->purge_range_hi[k] <= m->purge_range_hi[k - 1]) { c->err = "purge_range_hi must ascend"; return B200C_EINVAL; }
-    if (c->cancel.exchange(0)) { c->err = "cancelled"; return B200C_ECANCELLED; }        // stop requested before the task got here
-    // the rest of the sstable (Filter.db / Summary.db / Statistics.db side band / first+last key): single-output compactions
-    const b200c_output& o0 = res->outputs[0];
-    const bool want_meta = o0.key_buf || o0.filter || o0.summary || o0.stats;
-    if (want_meta && (m->max_sstable_bytes != 0 || getenv("B200C_K4_TWO_PASS"))) { c->err = "metadata side band with multi-file output"; return B200C_EUNSUPPORTED; }
-    if (want_meta && o0.filter && m->bloom_words && (m->bloom_hash_count <= 0 || m->bloom_words > (1ull << 31))) { c->err = "bloom geometry"; return B200C_EINVAL; }
-    if (m->ninputs > MAXK) { c->err = "more than 64 inputs per call"; return B200C_EUNSUPPORTED; }
-    if (m->tombstone_option != 0 || m->enforce_strict_liveness) { c->err = "tombstone_option / strict liveness"; return B200C_EUNSUPPORTED; }
-    if (m->nstatic_columns < 0 || m->nstatic_columns > MAXSTAT) { c->err = "more than 16 static columns"; return B200C_EUNSUPPORTED; }
-    if (m->nclustering > MAXCLUST || m->ncolumns >= 64 || m->ncolumns < 0) { c->err = "schema outside the supported envelope"; return B200C_EUNSUPPORTED; }
-    for (int k = 0; k < m->nstatic_columns; k++) if ((m->static_columns[k].type >> 8) & 0xFF) { c->err = "multi-cell static column"; return B200C_EUNSUPPORTED; }
-    if (res->noutputs_cap < 1 || !res->outputs) { c->err = "no output slot"; return B200C_EINVAL; }
-    if (m->out_chunk_len <= 0 || m->out_chunk_len > 65536 || (m->out_chunk_len & (m->out_chunk_len - 1))) { c->err = "output chunk_len"; return B200C_EUNSUPPORTED; }
-    const bool dev = flags & B200C_FLAG_DEVICE_PTRS;
-    const bool lcs = m->max_sstable_bytes != 0;
-    const int K = m->ninputs;
-    // whatever way this call ends, nothing may still be copying from or into the caller's buffers
-    struct CopyGuard { b200c_ctx* c; cudaStream_t main; ~CopyGuard() { c->stream = main; cudaStreamSynchronize(c->stream5); cudaStreamSynchronize(c->copy_stream); cudaStreamSynchronize(c->copy_out); } } copy_guard{c, c->stream};
+static_assert(MAXK == B200C_MAX_INPUTS && sizeof(RunStats) == sizeof(Pinned::run_stats) && sizeof(RunStats) == sizeof(Pinned::file_stats), "pinned read-backs");
+
+// K4 over the entries [lo, hi) of one fan-in class of the sorted list: one thread per partition, NT a block ...
+template <int M_CAP, int NT, bool CX = false> int k4_thr(b200c_ctx* c, const K4Args& ka, bool emit, uint64_t lo, uint64_t hi, size_t smem) {
+    if (hi <= lo) return B200C_OK;
+    const unsigned grid = (unsigned)((hi - lo + NT - 1) / NT);
+    if (emit) B200C_LAUNCH(c, (k_partition_thr<M_CAP, NT, true, CX>), grid, NT, smem, ka, lo, hi);
+    else if constexpr (!CX) B200C_LAUNCH(c, (k_partition_thr<M_CAP, NT, false>), grid, NT, smem, ka, lo, hi);
+    return B200C_OK;
+}
+// ... or one warp per partition, four a block
+template <int S> int k4_warp(b200c_ctx* c, const K4Args& ka, bool emit, uint64_t lo, uint64_t hi, size_t smem) {
+    if (hi <= lo) return B200C_OK;
+    if (emit) B200C_LAUNCH(c, (k_partition_warp<S, true>), (unsigned)((hi - lo + 3) / 4), 128, smem, ka, lo, hi);
+    else B200C_LAUNCH(c, (k_partition_warp<S, false>), (unsigned)((hi - lo + 3) / 4), 128, smem, ka, lo, hi);
+    return B200C_OK;
+}
+// > 48 KiB of dynamic shared memory needs an explicit opt-in. carveout (B200C_K4_CARVEOUT): percent of the SM's unified L1/shared memory
+// left to shared memory (A/B: fewer resident blocks, more L1 for the scattered reads of Data.db); unset: the driver sizes the carve-out
+// for the most blocks that fit
+template <int M_CAP, int NT, bool EMIT, bool CX = false> void k4_attr(size_t smem, const char* carveout = nullptr) {
+    cudaFuncSetAttribute(k_partition_thr<M_CAP, NT, EMIT, CX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (carveout) cudaFuncSetAttribute(k_partition_thr<M_CAP, NT, EMIT, CX>, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(carveout));
+}
+
+// staged K4 (A/B, DESIGN §3.1): one block per tile
+template <bool WIDE> int k4_staged(b200c_ctx* c, const K4Args& ka, uint64_t ntiles, size_t smem, const uint32_t* tstart, const uint8_t* big) {
+    B200C_LAUNCH(c, k_partition_staged<WIDE>, (unsigned)ntiles, ST_THREADS, smem, ka, tstart, big);
+    return B200C_OK;
+}
+template <bool WIDE> void k4_staged_attr(size_t smem) { cudaFuncSetAttribute(k_partition_staged<WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }
+
+struct CompactCall {
+    // ---- what the call was given
+    b200c_ctx* const c; const b200c_manifest* const m; b200c_result* const res;
+    const bool dev, lcs; const int K;
+    const bool raw_out, to_host_stream;            // compression disabled: Data.db + CRC.db (k_raw_checksum); one output file in host memory
+    const cudaMemcpyKind in_kind;                  // where the inputs come from
+    Pinned* const P; const cudaStream_t st, cs;    // read-backs; the main stream and the inputs' copy stream
+    const std::chrono::steady_clock::time_point t_start = std::chrono::steady_clock::now();
+    bool want_meta = false, two_pass = false;
+    int rc = B200C_OK;                             // what the call returns once it has run to its end (an output buffer too small)
+
+    // ---- its plan
+    struct Need { uint64_t h2d_a, h2d_b, k1_a, k1_b; };
+    bool have_summaries = true, sliced = false, deferred = false, istream = false;
+    int nr = 1;
+    std::vector<IdxSlice> isl;                     // the call's Index.db slice of every input
+    std::vector<int64_t> T;                        // piece r merges the partitions with token in (T[r], T[r + 1]]
+    std::vector<std::vector<IdxSlice>> psl;        // per piece and input: Index.db slice ...
+    std::vector<uint64_t> pustart;                 // ... and where the Data.db bytes its entries describe start ([ustart, slice.uend))
+    std::vector<std::vector<uint64_t>> psb;        // per piece and input: first of its Summary.db positions in d_summ
+    std::vector<Need> need;                        // per piece and input: chunks to copy (deferred mode) and to decompress
+    std::vector<uint64_t> range_bytes, range_end;  // per piece: input bytes; per piece and input: Data.db position behind the piece (scanner accounting)
+    std::vector<uint64_t> h2d_next, k1_next;       // deferred mode: first chunk of input i not yet copied / not yet decompressed
+    std::vector<std::vector<uint64_t>> co_host;    // chunk offsets of device-resident inputs taking the piece route
+    std::vector<uint64_t> ubase, ibase, cbase, obase, bbase;
+    uint64_t uo = 0, io = 0, co = 0, oo = 0, in_bytes = 0, bytes_read = 0;
+    CParams hp; std::vector<InDesc> hin;
+
+    // ---- device arrays
+    uint8_t *U = nullptr, *CD = nullptr, *IDX = nullptr; uint64_t *CO = nullptr, *d_bbase = nullptr, *d_summ = nullptr; CParams* dP = nullptr;
+    DevErr* d_err = nullptr; ChunkErr* d_cerr = nullptr; RunStats* d_stats = nullptr; unsigned long long *d_hist = nullptr, *d_rbytes = nullptr;
+    std::vector<const uint8_t*> k1_data, k1_tail; std::vector<const uint64_t*> k1_offs; std::vector<uint64_t> k1_tail_off; std::vector<K1Seg> segs;
+    int k1_batch_env = 0;
+    // metadata state (meta.cuh), device resident across the pieces of the call
+    StatGlobal* d_sg = nullptr; TdropTable* d_td = nullptr; uint32_t* d_bloom = nullptr; uint8_t *d_mkeys = nullptr, *d_sument = nullptr; uint64_t* d_sumoff = nullptr;
+    uint64_t written_total = 0, samples_total = 0, sument_bound = 0, bloom_words = 0; uint32_t meta_interval = 128;
+    // K2: partitions of every input
+    uint64_t total_parts = 0, slow_inputs = 0; std::vector<uint64_t> pcount, pbase;
+    int64_t* d_tok = nullptr; uint64_t *d_kp = nullptr, *d_upos = nullptr, *d_pbase = nullptr, *d_pcount = nullptr, *d_range = nullptr; uint16_t* d_klen = nullptr;
+    // per piece; the arrays of the last piece outlive the loop (the single-output writers work on them)
+    OutStream os; uint64_t L = 0;
+    uint64_t ubase_total = 0, ilen_total = 0, ncontrib_total = 0, nparts_total = 0;
+    uint64_t tail_len = 0; const uint8_t* tail_ptr = nullptr;      // bytes of the merged stream not yet handed to K5 (< one chunk)
+    bool index_fits = true;
+    uint64_t nparts = 0, ulen_out = 0, ilen_out = 0, n_le8 = 0, n_le12 = 0, n_le16 = 0, n_le32 = 0;
+    uint64_t *d_contrib = nullptr, *d_opfirst = nullptr, *d_bound = nullptr, *d_bpos = nullptr, *d_ioff = nullptr, *d_dsize = nullptr, *d_dpos = nullptr, *d_ipos = nullptr, *d_wrank = nullptr;
+    uint32_t *d_list = nullptr, *d_icap = nullptr, *d_insz = nullptr, *d_ipay = nullptr, *d_nblk = nullptr, *d_ihead = nullptr, *d_isize = nullptr;
+    uint32_t *d_stmunf = nullptr, *d_strows = nullptr, *d_ccount = nullptr, *d_wflag = nullptr; uint8_t *d_ovf = nullptr, *d_big = nullptr;
+    uint8_t *UOUT = nullptr, *IOUT = nullptr, *ISCR = nullptr, *SCRATCH = nullptr;
+    size_t smem8 = 0, smem12 = 0, smem16 = 0, smem64 = 0, cell_smem32 = 0;
+    K4Args ka;
+    // multi-file output
+    int lcs_stride = 0; uint8_t* slots = nullptr; uint32_t *file_len = nullptr, *seg_raw = nullptr; uint64_t *woffs = nullptr, *d_cut = nullptr;
+    // stage clock: marks on the main stream; the time between two marks is charged to the stage of the first
+    struct Mark { int stage; cudaEvent_t ev; };
+    std::vector<Mark> marks;
+
+    CompactCall(b200c_ctx* c_, const b200c_manifest* m_, b200c_result* res_, int flags)
+        : c(c_), m(m_), res(res_), dev((flags & B200C_FLAG_DEVICE_PTRS) != 0), lcs(m_->max_sstable_bytes != 0), K(m_->ninputs),
+          raw_out(m_->out_compressor == COMP_UNCOMPRESSED), to_host_stream(!dev && !lcs), in_kind(dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice),
+          P(c_->h_pinned), st(c_->stream), cs(c_->copy_stream) {
+        cudaSetDevice(c->device);
+        c->prog_stage.store(0); c->prog_scanned.store(0);
+        for (int i = 0; i < B200C_MAX_INPUTS; i++) c->prog_input_pos[i].store(0);
+        c->prog_seq.fetch_add(1);              // after the resets: figures read behind a new call_seq belong to this call
+    }
+    // whatever way the call ends, the stage clock is closed and nothing still reads or writes the caller's buffers
+    ~CompactCall() {
+        if (c->timing) timing_end(c);
+        cudaStreamSynchronize(st); cudaStreamSynchronize(cs); cudaStreamSynchronize(c->copy_out);
+    }
+
+    int corrupt(int input, int kind, uint64_t chunk, uint64_t offset, std::string msg) {
+        res->corruption.input = input; res->corruption.kind = kind; res->corruption.chunk = chunk; res->corruption.offset = offset;
+        c->err = std::move(msg);
+        return B200C_ECORRUPT;
+    }
+    int chunk_error(uint64_t word) {                  // word = d_cerr: (input << 48 | chunk << 8 | kind)
+        const int which = (int)(word >> 48), kind = (int)(word & 0xff); const uint64_t chunk = (word >> 8) & 0xFFFFFFFFFFull;
+        // an uncompressed input's chunk starts at chunk * chunk_len of Data.db
+        const uint64_t off = which < K && m->inputs[which].compressor == COMP_UNCOMPRESSED ? chunk * (uint64_t)m->inputs[which].chunk_len : 0;
+        return corrupt(which, kind, chunk, off, std::string(kind == 1 ? "chunk CRC mismatch" : "malformed compressed chunk") + " in input " + std::to_string(which) + " chunk " + std::to_string(chunk));
+    }
+    int index_data_mismatch(uint64_t word) {
+        const int in = (int)((word >> 48) & 0xFF);
+        return corrupt(in, 3, 0, word & 0xFFFFFFFFFFFFull, "Index.db does not match Data.db in input " + std::to_string(in));
+    }
+    // the request is consumed by the call that reports it (b200c.h: sticky until then, so one that lands before the call is not lost)
+    int check_cancel() { if (c->cancel.exchange(0)) { c->err = "cancelled"; return B200C_ECANCELLED; } return B200C_OK; }
+    void mark(int stage) {
+        const size_t k = marks.size();
+        if (k >= c->ev_marks.size()) { cudaEvent_t e; cudaEventCreate(&e); c->ev_marks.push_back(e); }
+        cudaEventRecord(c->ev_marks[k], st); marks.push_back(Mark{stage, c->ev_marks[k]});
+    }
+    void finish_marks() {
+        for (int k = 0; k < 8; k++) c->stage_ms[k] = 0;
+        for (size_t k = 0; k + 1 < marks.size(); k++) { float ms = 0; cudaEventElapsedTime(&ms, marks[k].ev, marks[k + 1].ev); if (marks[k].stage >= 0) c->stage_ms[marks[k].stage] += ms; }
+        c->nstages = 6;
+    }
+
+    int validate() {
+        if (m->abi_version != B200C_ABI_VERSION || m->ninputs <= 0) { c->err = "bad manifest"; return B200C_EINVAL; }
+        if (m->partitioner != B200C_PARTITIONER_MURMUR3 && m->partitioner != B200C_PARTITIONER_BYTE_ORDERED) { c->err = "partitioner not supported (Murmur3Partitioner and ByteOrderedPartitioner are)"; return B200C_EUNSUPPORTED; }
+        if (m->partitioner == B200C_PARTITIONER_BYTE_ORDERED && (m->token_lo != INT64_MIN || m->token_hi != INT64_MAX || m->npurge_ranges)) { c->err = "ByteOrderedPartitioner: token sub-ranges are not expressible"; return B200C_EUNSUPPORTED; }
+        if (m->npurge_ranges < 0 || (m->npurge_ranges && (!m->purge_range_hi || !m->purge_range_max_ts))) { c->err = "purge table"; return B200C_EINVAL; }
+        for (int k = 1; k < m->npurge_ranges; k++) if (m->purge_range_hi[k] <= m->purge_range_hi[k - 1]) { c->err = "purge_range_hi must ascend"; return B200C_EINVAL; }
+        if (c->cancel.exchange(0)) { c->err = "cancelled"; return B200C_ECANCELLED; }        // stop requested before the task got here
+        // the rest of the sstable (Filter.db / Summary.db / Statistics.db side band / first+last key): single-output compactions
+        const b200c_output& o0 = res->outputs[0];
+        want_meta = o0.key_buf || o0.filter || o0.summary || o0.stats;
+        if (want_meta && (m->max_sstable_bytes != 0 || getenv("B200C_K4_TWO_PASS"))) { c->err = "metadata side band with multi-file output"; return B200C_EUNSUPPORTED; }
+        if (want_meta && o0.filter && m->bloom_words && (m->bloom_hash_count <= 0 || m->bloom_words > (1ull << 31))) { c->err = "bloom geometry"; return B200C_EINVAL; }
+        if (m->ninputs > MAXK) { c->err = "more than 64 inputs per call"; return B200C_EUNSUPPORTED; }
+        if (m->tombstone_option != 0 || m->enforce_strict_liveness) { c->err = "tombstone_option / strict liveness"; return B200C_EUNSUPPORTED; }
+        if (m->nstatic_columns < 0 || m->nstatic_columns > MAXSTAT) { c->err = "more than 16 static columns"; return B200C_EUNSUPPORTED; }
+        if (m->nclustering > MAXCLUST || m->ncolumns >= 64 || m->ncolumns < 0) { c->err = "schema outside the supported envelope"; return B200C_EUNSUPPORTED; }
+        for (int k = 0; k < m->nstatic_columns; k++) if ((m->static_columns[k].type >> 8) & 0xFF) { c->err = "multi-cell static column"; return B200C_EUNSUPPORTED; }
+        if (res->noutputs_cap < 1 || !res->outputs) { c->err = "no output slot"; return B200C_EINVAL; }
+        if (m->out_chunk_len <= 0 || m->out_chunk_len > 65536 || (m->out_chunk_len & (m->out_chunk_len - 1))) { c->err = "output chunk_len"; return B200C_EUNSUPPORTED; }
+        for (int i = 0; i < K; i++) {
+            const b200c_input& in = m->inputs[i];
+            if (in.chunk_len <= 0 || in.chunk_len > 65536 || (in.chunk_len & (in.chunk_len - 1))) { c->err = "input chunk_len"; return B200C_EUNSUPPORTED; }
+            if (in.ncolumns < 0 || in.ncolumns >= 64) { c->err = "input columns"; return B200C_EUNSUPPORTED; }
+            if (in.nchunks != (in.data_length + in.chunk_len - 1) / (uint64_t)in.chunk_len) { c->err = "chunk count does not match data_length"; return B200C_EINVAL; }
+            if (in.compressor != COMP_LZ4 && !comp_is_snappy(in.compressor) && in.compressor != COMP_NONE && in.compressor != COMP_UNCOMPRESSED) { c->err = "unknown compressor"; return B200C_EINVAL; }
+            if (in.compressor == COMP_UNCOMPRESSED && in.data_len != in.data_length) { c->err = "uncompressed input: data_length must equal data_len"; return B200C_EINVAL; }
+            for (int k = 0; k < in.ncolumns; k++) if (in.column_map[k] < 0 || in.column_map[k] >= m->ncolumns || (k && in.column_map[k] <= in.column_map[k - 1])) { c->err = "column_map must be strictly increasing (both headers are name ordered)"; return B200C_EINVAL; }
+            if (in.nstatic_columns < 0 || in.nstatic_columns > m->nstatic_columns) { c->err = "input static columns"; return B200C_EINVAL; }
+            for (int k = 0; k < in.nstatic_columns; k++) if (in.static_column_map[k] < 0 || in.static_column_map[k] >= m->nstatic_columns || (k && in.static_column_map[k] <= in.static_column_map[k - 1])) { c->err = "static_column_map must be strictly increasing"; return B200C_EINVAL; }
+        }
+        return B200C_OK;
+    }
 
     // ---- Index.db slices: a token sub-range with Summary.db samples touches only its part of every Index.db ------------------------------
-    bool have_summaries = true;
-    for (int i = 0; i < K; i++) if (m->inputs[i].index_len && !(m->inputs[i].summary_positions && m->inputs[i].nsummary)) have_summaries = false;
-    const bool sliced = have_summaries && !lcs && (m->token_lo != INT64_MIN || m->token_hi != INT64_MAX) && !getenv("B200C_NO_INDEX_SLICES");
-    std::vector<IdxSlice> isl(K);
-    for (int i = 0; i < K; i++) isl[i] = IdxSlice{0, m->inputs[i].index_len, m->inputs[i].data_length, 0, have_summaries ? m->inputs[i].nsummary : 0};
-    if (sliced) {
+    int plan_slices() {
+        for (int i = 0; i < K; i++) if (m->inputs[i].index_len && !(m->inputs[i].summary_positions && m->inputs[i].nsummary)) have_summaries = false;
+        sliced = have_summaries && !lcs && (m->token_lo != INT64_MIN || m->token_hi != INT64_MAX) && !getenv("B200C_NO_INDEX_SLICES");
+        isl.resize(K);
+        for (int i = 0; i < K; i++) isl[i] = IdxSlice{0, m->inputs[i].index_len, m->inputs[i].data_length, 0, have_summaries ? m->inputs[i].nsummary : 0};
+        if (!sliced) return B200C_OK;
         if (!dev) {
             for (int i = 0; i < K; i++) { const b200c_input& in = m->inputs[i];
-                if (in.index_len && !compute_index_slice(in.index, in.index_len, in.summary_positions, in.nsummary, in.data_length, m->partitioner, m->token_lo, m->token_hi, &isl[i])) {
-                    c->err = "Summary.db positions of input " + std::to_string(i) + " do not point at Index.db entries"; res->corruption.input = i; res->corruption.kind = 3; res->corruption.chunk = 0; res->corruption.offset = 0; return B200C_ECORRUPT; } }
-        } else {
-            uint8_t* w; B200C_TRY(ws_typed(c, WS_SLICE, (size_t)K * (8 * 5 + sizeof(IdxSlice) + 4) + 64, &w));
-            std::vector<uint64_t> hv((size_t)K * 5);
-            for (int i = 0; i < K; i++) { const b200c_input& in = m->inputs[i]; hv[i] = (uint64_t)(uintptr_t)in.index; hv[K + i] = in.index_len; hv[2 * K + i] = (uint64_t)(uintptr_t)in.summary_positions; hv[3 * K + i] = in.nsummary; hv[4 * K + i] = in.data_length; }
-            uint64_t* dv = (uint64_t*)w; IdxSlice* dsl = (IdxSlice*)(dv + 5 * K); uint32_t* dok = (uint32_t*)(dsl + K);
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(dv, hv.data(), hv.size() * 8, cudaMemcpyHostToDevice, c->stream));
-            k_index_slices<<<(K + 63) / 64, 64, 0, c->stream>>>((const uint8_t* const*)dv, dv + K, (const uint64_t* const*)(dv + 2 * K), dv + 3 * K, dv + 4 * K, K, m->partitioner, m->token_lo, m->token_hi, dsl, dok);
-            std::vector<uint32_t> ok(K);
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(isl.data(), dsl, sizeof(IdxSlice) * K, cudaMemcpyDeviceToHost, c->stream));
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(ok.data(), dok, 4 * K, cudaMemcpyDeviceToHost, c->stream));
-            B200C_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-            for (int i = 0; i < K; i++) if (m->inputs[i].index_len && !ok[i]) { c->err = "Summary.db positions of input " + std::to_string(i) + " do not point at Index.db entries"; res->corruption.input = i; res->corruption.kind = 3; res->corruption.chunk = 0; res->corruption.offset = 0; return B200C_ECORRUPT; }
-                         else if (!m->inputs[i].index_len) isl[i] = IdxSlice{0, 0, m->inputs[i].data_length, 0, 0};
+                if (in.index_len && !compute_index_slice(in.index, in.index_len, in.summary_positions, in.nsummary, in.data_length, m->partitioner, m->token_lo, m->token_hi, &isl[i]))
+                    return corrupt(i, 3, 0, 0, "Summary.db positions of input " + std::to_string(i) + " do not point at Index.db entries"); }
+            return B200C_OK;
         }
+        uint8_t* w; B200C_TRY(ws_typed(c, WS_SLICE, (size_t)K * (8 * 5 + sizeof(IdxSlice) + 4) + 64, &w));
+        std::vector<uint64_t> hv((size_t)K * 5);
+        for (int i = 0; i < K; i++) { const b200c_input& in = m->inputs[i]; hv[i] = (uint64_t)(uintptr_t)in.index; hv[K + i] = in.index_len; hv[2 * K + i] = (uint64_t)(uintptr_t)in.summary_positions; hv[3 * K + i] = in.nsummary; hv[4 * K + i] = in.data_length; }
+        uint64_t* dv = (uint64_t*)w; IdxSlice* dsl = (IdxSlice*)(dv + 5 * K); uint32_t* dok = (uint32_t*)(dsl + K);
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(dv, hv.data(), hv.size() * 8, cudaMemcpyHostToDevice, st));
+        k_index_slices<<<(K + 63) / 64, 64, 0, st>>>((const uint8_t* const*)dv, dv + K, (const uint64_t* const*)(dv + 2 * K), dv + 3 * K, dv + 4 * K, K, m->partitioner, m->token_lo, m->token_hi, dsl, dok);
+        std::vector<uint32_t> ok(K);
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(isl.data(), dsl, sizeof(IdxSlice) * K, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(ok.data(), dok, 4 * K, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
+        for (int i = 0; i < K; i++) if (m->inputs[i].index_len && !ok[i]) return corrupt(i, 3, 0, 0, "Summary.db positions of input " + std::to_string(i) + " do not point at Index.db entries");
+                                 else if (!m->inputs[i].index_len) isl[i] = IdxSlice{0, 0, m->inputs[i].data_length, 0, 0};
+        return B200C_OK;
     }
 
     // ---- layout of the concatenated device buffers -------------------------------------------------------------------------------
-    std::vector<uint64_t> ubase(K + 1), ibase(K + 1), cbase(K + 1), obase(K + 1), bbase(K + 1);
-    CParams hp; memset(&hp, 0, sizeof(hp));
-    std::vector<InDesc> hin(K); memset(hin.data(), 0, sizeof(InDesc) * K);
-    uint64_t uo = 0, io = 0, co = 0, oo = 0, bo = 0, in_bytes = 0;
-    for (int i = 0; i < K; i++) {
-        const b200c_input& in = m->inputs[i];
-        if (in.chunk_len <= 0 || in.chunk_len > 65536 || (in.chunk_len & (in.chunk_len - 1))) { c->err = "input chunk_len"; return B200C_EUNSUPPORTED; }
-        if (in.ncolumns < 0 || in.ncolumns >= 64) { c->err = "input columns"; return B200C_EUNSUPPORTED; }
-        if (in.nchunks != (in.data_length + in.chunk_len - 1) / (uint64_t)in.chunk_len) { c->err = "chunk count does not match data_length"; return B200C_EINVAL; }
-        if (in.compressor != COMP_LZ4 && !comp_is_snappy(in.compressor) && in.compressor != COMP_NONE && in.compressor != COMP_UNCOMPRESSED) { c->err = "unknown compressor"; return B200C_EINVAL; }
-        if (in.compressor == COMP_UNCOMPRESSED && in.data_len != in.data_length) { c->err = "uncompressed input: data_length must equal data_len"; return B200C_EINVAL; }
-        ubase[i] = uo; uo += (in.data_length + 64 + 65535) & ~65535ull;
-        const uint64_t ilen_i = isl[i].hi - isl[i].lo;               // Index.db bytes this call reads from input i
-        ibase[i] = io; io += (ilen_i + 64 + 255) & ~255ull;       // 256-aligned, >= 64 bytes behind every input: K2's 16-byte reads need IW_PAD
-        // uncompressed inputs are copied from the host straight into U (no staging in CD); `in_bytes` counts every input for the piece schedule
-        cbase[i] = co; if (in.compressor != COMP_UNCOMPRESSED) co += (in.data_len + 64 + 255) & ~255ull;
-        in_bytes += (in.data_len + 64 + 255) & ~255ull;
-        obase[i] = oo; oo += in.nchunks + 1;
-        bbase[i] = bo; bo += (ilen_i + IB - 1) / IB;
-        InDesc& d = hin[i];
-        d.ubase = ubase[i]; d.ulen = in.data_length; d.ibase = ibase[i]; d.ilen = ilen_i; d.uend = isl[i].uend;
-        d.min_ts = in.header_stats.min_timestamp; d.min_ldt = in.header_stats.min_local_deletion_time; d.min_ttl = in.header_stats.min_ttl;
-        d.ncols = in.ncolumns;
-        for (int k = 0; k < in.ncolumns; k++) {
-            if (in.column_map[k] < 0 || in.column_map[k] >= m->ncolumns || (k && in.column_map[k] <= in.column_map[k - 1])) { c->err = "column_map must be strictly increasing (both headers are name ordered)"; return B200C_EINVAL; }
-            d.colmap[k] = in.column_map[k];
+    int layout() {
+        ubase.assign(K + 1, 0); ibase.assign(K + 1, 0); cbase.assign(K + 1, 0); obase.assign(K + 1, 0); bbase.assign(K + 1, 0);
+        memset(&hp, 0, sizeof(hp));
+        hin.resize(K); memset(hin.data(), 0, sizeof(InDesc) * K);
+        uint64_t bo = 0;
+        for (int i = 0; i < K; i++) {
+            const b200c_input& in = m->inputs[i];
+            ubase[i] = uo; uo += (in.data_length + 64 + 65535) & ~65535ull;
+            const uint64_t ilen_i = isl[i].hi - isl[i].lo;               // Index.db bytes this call reads from input i
+            ibase[i] = io; io += (ilen_i + 64 + 255) & ~255ull;       // 256-aligned, >= 64 bytes behind every input: K2's 16-byte reads need IW_PAD
+            // uncompressed inputs are copied from the host straight into U (no staging in CD); `in_bytes` counts every input for the piece schedule
+            cbase[i] = co; if (in.compressor != COMP_UNCOMPRESSED) co += (in.data_len + 64 + 255) & ~255ull;
+            in_bytes += (in.data_len + 64 + 255) & ~255ull;
+            obase[i] = oo; oo += in.nchunks + 1;
+            bbase[i] = bo; bo += (ilen_i + IB - 1) / IB;
+            InDesc& d = hin[i];
+            d.ubase = ubase[i]; d.ulen = in.data_length; d.ibase = ibase[i]; d.ilen = ilen_i; d.uend = isl[i].uend;
+            d.min_ts = in.header_stats.min_timestamp; d.min_ldt = in.header_stats.min_local_deletion_time; d.min_ttl = in.header_stats.min_ttl;
+            d.ncols = in.ncolumns;
+            for (int k = 0; k < in.ncolumns; k++) d.colmap[k] = in.column_map[k];
+            d.nstat = in.nstatic_columns; d._pad = 0;
+            for (int k = 0; k < in.nstatic_columns; k++) d.smap[k] = in.static_column_map[k];
         }
-        d.nstat = in.nstatic_columns; d._pad = 0;
-        if (in.nstatic_columns < 0 || in.nstatic_columns > m->nstatic_columns) { c->err = "input static columns"; return B200C_EINVAL; }
-        for (int k = 0; k < in.nstatic_columns; k++) {
-            if (in.static_column_map[k] < 0 || in.static_column_map[k] >= m->nstatic_columns || (k && in.static_column_map[k] <= in.static_column_map[k - 1])) { c->err = "static_column_map must be strictly increasing"; return B200C_EINVAL; }
-            d.smap[k] = in.static_column_map[k];
+        ubase[K] = uo; ibase[K] = io; cbase[K] = co; obase[K] = oo; bbase[K] = bo;
+        if (uo >= (1ull << 40)) { c->err = "decompressed inputs of 1 TiB or more per call"; return B200C_EUNSUPPORTED; }      // stream offsets are 40-bit in the K4 cursors
+        hp.ninputs = K; hp.nclust = m->nclustering; hp.ncols = m->ncolumns; hp.column_index_size = m->column_index_size > 0 ? m->column_index_size : 65536;
+        for (int k = 0; k < m->nclustering; k++) { hp.ctype[k] = m->clustering[k].type; hp.cfix[k] = m->clustering[k].fixed_len; }
+        for (int k = 0; k < m->ncolumns; k++) {                 // multi-cell columns: include/b200c.h B200C_COLUMN_COMPLEX / _FIXED; they follow the simple ones
+            const int ptype = ((m->columns[k].type >> 8) & 0xFF) - 1;
+            hp.vfix[k] = m->columns[k].fixed_len & 0xFFFF;
+            if (ptype >= 0) {
+                if (ptype > TYPE_TIMEUUID) { c->err = "cell path class"; return B200C_EINVAL; }
+                if (hp.ncx >= MAXCX) { c->err = "more than 8 multi-cell columns"; return B200C_EUNSUPPORTED; }
+                if (!hp.ncx) hp.cx_first = k;
+                hp.ptype[hp.ncx] = ptype; hp.pfix[hp.ncx] = (int32_t)((uint32_t)m->columns[k].fixed_len >> 16); hp.ncx++;
+            } else if (hp.ncx) { c->err = "simple column behind a multi-cell one (ColumnMetadata order: simple columns first)"; return B200C_EINVAL; }
+            if ((m->columns[k].type & 0xFF) == B200C_TYPE_COUNTER) {      // counter columns: cells merged shard by shard (partition.cuh ctr_merge), CX kernels
+                if (ptype >= 0) { c->err = "collection of counters"; return B200C_EINVAL; }
+                hp.ctr_mask |= 1ull << k;
+            }
         }
+        if (!hp.ncx) hp.cx_first = m->ncolumns;
+        for (int k = 0; k < m->nstatic_columns; k++) if ((m->static_columns[k].type & 0xFF) == B200C_TYPE_COUNTER) hp.sctr_mask |= 1ull << k;
+        hp.nstat = m->nstatic_columns; hp.mcols = std::max(m->ncolumns, m->nstatic_columns);
+        for (int k = 0; k < m->nstatic_columns; k++) hp.sfix[k] = m->static_columns[k].fixed_len;
+        hp.o_min_ts = m->out_stats.min_timestamp; hp.o_min_ldt = m->out_stats.min_local_deletion_time; hp.o_min_ttl = m->out_stats.min_ttl;
+        hp.now = m->now_in_sec; hp.gc_before = m->gc_before; hp.purge_max_ts = m->purge_max_timestamp;
+        hp.partitioner = m->partitioner;
+        return B200C_OK;
     }
-    ubase[K] = uo; ibase[K] = io; cbase[K] = co; obase[K] = oo; bbase[K] = bo;
-    if (uo >= (1ull << 40)) { c->err = "decompressed inputs of 1 TiB or more per call"; return B200C_EUNSUPPORTED; }      // stream offsets are 40-bit in the K4 cursors
-    (void)bo;
-    hp.ninputs = K; hp.nclust = m->nclustering; hp.ncols = m->ncolumns; hp.column_index_size = m->column_index_size > 0 ? m->column_index_size : 65536;
-    for (int k = 0; k < m->nclustering; k++) { hp.ctype[k] = m->clustering[k].type; hp.cfix[k] = m->clustering[k].fixed_len; }
-    for (int k = 0; k < m->ncolumns; k++) {                 // multi-cell columns: include/b200c.h B200C_COLUMN_COMPLEX / _FIXED; they follow the simple ones
-        const int ptype = ((m->columns[k].type >> 8) & 0xFF) - 1;
-        hp.vfix[k] = m->columns[k].fixed_len & 0xFFFF;
-        if (ptype >= 0) {
-            if (ptype > TYPE_TIMEUUID) { c->err = "cell path class"; return B200C_EINVAL; }
-            if (hp.ncx >= MAXCX) { c->err = "more than 8 multi-cell columns"; return B200C_EUNSUPPORTED; }
-            if (!hp.ncx) hp.cx_first = k;
-            hp.ptype[hp.ncx] = ptype; hp.pfix[hp.ncx] = (int32_t)((uint32_t)m->columns[k].fixed_len >> 16); hp.ncx++;
-        } else if (hp.ncx) { c->err = "simple column behind a multi-cell one (ColumnMetadata order: simple columns first)"; return B200C_EINVAL; }
-        if ((m->columns[k].type & 0xFF) == B200C_TYPE_COUNTER) {      // counter columns: cells merged shard by shard (partition.cuh ctr_merge), CX kernels
-            if (ptype >= 0) { c->err = "collection of counters"; return B200C_EINVAL; }
-            hp.ctr_mask |= 1ull << k;
-        }
-    }
-    if (!hp.ncx) hp.cx_first = m->ncolumns;
-    for (int k = 0; k < m->nstatic_columns; k++) if ((m->static_columns[k].type & 0xFF) == B200C_TYPE_COUNTER) hp.sctr_mask |= 1ull << k;
-    hp.nstat = m->nstatic_columns; hp.mcols = std::max(m->ncolumns, m->nstatic_columns);
-    for (int k = 0; k < m->nstatic_columns; k++) hp.sfix[k] = m->static_columns[k].fixed_len;
-    hp.o_min_ts = m->out_stats.min_timestamp; hp.o_min_ldt = m->out_stats.min_local_deletion_time; hp.o_min_ttl = m->out_stats.min_ttl;
-    hp.now = m->now_in_sec; hp.gc_before = m->gc_before; hp.purge_max_ts = m->purge_max_timestamp;
-    hp.partitioner = m->partitioner;
 
+    // ---- token-range pieces ----------------------------------------------------------------------------------------------------------
     // Token-range streaming (host buffers, one output file): Index.db goes to the device first; once K2 has turned it into tokens and
-    // positions the token space is cut into `want_ranges` pieces, the Data.db chunks each piece needs are copied piece by piece on the
-    // copy stream, and K1/K3/K4/K5 of piece r run underneath the copies of the pieces after it and the read-back of the pieces before
-    // it. Device-resident inputs and multi-file (LCS) outputs run as one piece.
-    // Piece boundaries as fractions of the token-sorted input: small pieces first (the kernels can start as soon as little data
-    // has arrived), doubling afterwards (few pieces = little per-piece overhead). B200C_RANGES=n forces n equal pieces (tests, tuning).
-    std::vector<double> cuts; bool forced_ranges = false;          // interior cut points in (0, 1)
-    if (!dev && !lcs) {
-        if (const char* e = getenv("B200C_RANGES")) {
-            int n = std::max(1, std::min((int)MAX_RANGES, atoi(e))); forced_ranges = true;
-            for (int r = 1; r < n; r++) cuts.push_back((double)r / n);
-        } else if (in_bytes >= (1536ull << 20)) {
-            // The kernels of a piece take longer than its copies, so the pipeline is kernel bound as long as no piece waits for its own
-            // data: a small first piece (the kernels start early), then EQUAL pieces. Doubling pieces (B200C_SCHEDULE=geometric) end with a
-            // piece of half the input that cannot start before the last byte has arrived, and the kernels idle until it has.
-            const double f0 = std::min(0.5, std::max(1.0 / 16, (double)(512ull << 20) / (double)in_bytes));
-            const char* sch = getenv("B200C_SCHEDULE");
-            if (sch && !strcmp(sch, "geometric")) { for (double f = f0; f < 1.0 && cuts.size() + 1 < MAX_RANGES; f *= 2) cuts.push_back(f); }
-            else {
+    // positions the token space is cut into pieces, the Data.db chunks each piece needs are copied piece by piece on the copy stream, and
+    // K1/K3/K4/K5 of piece r run underneath the copies of the pieces after it and the read-back of the pieces before it. Device-resident
+    // inputs and multi-file (LCS) outputs run as one piece.
+    void plan_pieces() {
+        std::vector<double> cuts; bool forced_ranges = false;          // interior cut points in (0, 1), as fractions of the token-sorted input
+        if (!dev && !lcs) {
+            if (const char* e = getenv("B200C_RANGES")) {              // B200C_RANGES=n forces n equal pieces (tests, tuning)
+                int n = std::max(1, std::min((int)MAX_RANGES, atoi(e))); forced_ranges = true;
+                for (int r = 1; r < n; r++) cuts.push_back((double)r / n);
+            } else if (in_bytes >= (1536ull << 20)) {
+                // The kernels of a piece take longer than its copies, so the pipeline is kernel bound as long as no piece waits for its own
+                // data: a small first piece (the kernels start early), then EQUAL pieces. Doubling pieces end with a piece of half the input
+                // that cannot start before the last byte has arrived, and the kernels idle until it has (DESIGN §3.4).
+                const double f0 = std::min(0.5, std::max(1.0 / 16, (double)(512ull << 20) / (double)in_bytes));
                 const double piece = std::max((double)in_bytes / 8, (double)(768ull << 20));
                 int n = (int)std::ceil((1.0 - f0) * (double)in_bytes / piece); n = std::max(1, std::min(n, (int)MAX_RANGES - 1));
                 for (int k = 0; k < n; k++) cuts.push_back(f0 + (1.0 - f0) * k / n);
             }
         }
+        // with Summary.db positions for every input the Index.db walk does not need Data.db: its copies are then scheduled after K2.
+        // Device-resident inputs take the same route when the call is a token sub-range: K2 first, then only the chunks the range crosses are decoded.
+        deferred = !lcs && have_summaries && (!dev || sliced);
+        T = {m->token_lo, m->token_hi}; psl.assign(1, isl); pustart.assign((size_t)K, 0);
+        if (deferred && !dev && !cuts.empty()) istream = cut_pieces(cuts, forced_ranges);
+        nr = (int)T.size() - 1;
     }
-    int want_ranges = (int)cuts.size() + 1;
-    // with Summary.db positions for every input the Index.db walk does not need Data.db: its copies are then scheduled after K2.
-    // Device-resident inputs take the same route when the call is a token sub-range: K2 first, then only the chunks the range crosses are decoded.
-    const bool deferred = !lcs && have_summaries && (!dev || sliced);
-    if (!deferred) { want_ranges = 1; cuts.clear(); }
     // Index.db streaming (host buffers, several pieces): the pieces are cut on the HOST, at tokens of Summary.db samples of the input with the
     // most samples, and every piece brings its own Index.db slices (the samples bracketing its token range, as a ranged scanner would seek),
     // its Summary positions and its Data.db chunks. K2 runs per piece: nothing waits for the whole Index.db (gigabytes of PCIe
     // copies on configs[1]) any more, and the per-partition arrays are piece sized.
-    std::vector<int64_t> T{m->token_lo, m->token_hi};
-    std::vector<std::vector<IdxSlice>> psl(1, isl);                 // per piece and input: Index.db slice ...
-    std::vector<uint64_t> pustart((size_t)K, 0);                    // ... and where the Data.db bytes its entries describe start ([ustart, slice.uend))
-    bool istream = false;
-    if (deferred && !dev && want_ranges > 1) {
-        // Summary.db is a hint here as everywhere: if its positions do not parse or the slices they give do not tile the call's own
-        // slice, the call runs as one piece (K2 over the whole Index.db, as before)
-        auto plan = [&]() -> bool {
-            int imax = 0; uint64_t nmax = 0;
-            for (int i = 0; i < K; i++) if (isl[i].s_count > nmax) { nmax = isl[i].s_count; imax = i; }
-            if (nmax < (uint64_t)want_ranges * (forced_ranges ? 1 : 32)) return false;
-            const b200c_input& big = m->inputs[imax];
-            std::vector<int64_t> t2{m->token_lo};
-            for (int r = 1; r < want_ranges; r++) {
-                const uint64_t sidx = isl[imax].s_first + std::min<uint64_t>(nmax - 1, (uint64_t)(nmax * cuts[r - 1]));
-                int64_t t = 0;
-                if (!sample_token(big.index, big.index_len, big.summary_positions[sidx], m->partitioner, &t)) return false;
-                if (t > t2.back() && t < m->token_hi) t2.push_back(t);
-            }
-            t2.push_back(m->token_hi);
-            const int n2 = (int)t2.size() - 1;
-            if (n2 < 2) return false;
-            std::vector<std::vector<IdxSlice>> p2(n2, isl); std::vector<uint64_t> u2((size_t)n2 * K, 0);
-            for (int r = 0; r < n2; r++) for (int i = 0; i < K; i++) {
-                const b200c_input& in = m->inputs[i];
-                IdxSlice& sl = p2[r][i];
-                if (!in.index_len) { sl = IdxSlice{0, 0, in.data_length, 0, 0}; u2[(size_t)r * K + i] = in.data_length; continue; }
-                if (!compute_index_slice(in.index, in.index_len, in.summary_positions, in.nsummary, in.data_length, m->partitioner, t2[r], t2[r + 1], &sl)) return false;
-                // every entry must lie in some piece's slice: consecutive slices touch or overlap, the first starts and the last ends with the call's own
-                if (r == 0 && sl.lo != isl[i].lo) return false;
-                if (r == n2 - 1 && sl.hi != isl[i].hi) return false;
-                if (r > 0 && (sl.lo > p2[r - 1][i].hi || sl.lo < p2[r - 1][i].lo || sl.hi < p2[r - 1][i].hi)) return false;
-                uint64_t pos = sl.uend;
-                if (sl.hi > sl.lo && !entry_data_position(in.index, in.index_len, sl.lo, in.data_length, &pos)) return false;
-                if (pos > sl.uend) return false;
-                u2[(size_t)r * K + i] = pos;
-            }
-            T = t2; psl = p2; pustart = u2;
-            return true;
-        };
-        istream = plan();
-    }
-    const int nr = (int)T.size() - 1;
-    uint8_t *U, *CD, *IDX; uint64_t* CO; CParams* dP; uint64_t* d_bbase; DevErr* d_err; ChunkErr* d_cerr; RunStats* d_stats; unsigned long long* d_hist;
-    B200C_TRY(ws_typed(c, WS_U, uo + 64, &U));
-    // K1's view of input i. Host inputs are staged in CD / CO (uncompressed ones go to U itself and are verified there). Device-resident inputs are read where the caller keeps them: no copy,
-    // no second image of the compressed inputs in device memory; only the file's tail is staged for the decoders' word reads (k1_src).
-    std::vector<const uint8_t*> k1_data(K), k1_tail(K, nullptr); std::vector<const uint64_t*> k1_offs(K); std::vector<uint64_t> k1_tail_off(K, ~0ull);
-    if (dev) {
-        std::vector<uint64_t> tb(K + 1, 0);
-        // (uncompressed inputs: the ingest kernel reads whole aligned words inside the file only, nothing to stage)
-        auto tail_window = [&](const b200c_input& in) -> uint64_t { return in.compressor == COMP_UNCOMPRESSED ? 0 : std::min(in.data_len, k1_tail_window(chunk_max_compressed(in.compressor, in.chunk_len), in.chunk_len)); };
-        for (int i = 0; i < K; i++) tb[i + 1] = tb[i] + ((tail_window(m->inputs[i]) + 64 + 15) & ~15ull);
-        uint8_t* TAIL; B200C_TRY(ws_typed(c, WS_K1TAIL, tb[K] + 64, &TAIL));
-        CD = nullptr; CO = nullptr;
-        for (int i = 0; i < K; i++) {
-            const b200c_input& in = m->inputs[i];
-            const uint64_t win = tail_window(in);
-            k1_data[i] = in.data; k1_offs[i] = in.chunk_offsets; k1_tail[i] = TAIL + tb[i]; k1_tail_off[i] = in.data_len - win;
-            if (win) B200C_CUDA_TRY(c, cudaMemcpyAsync(TAIL + tb[i], in.data + (in.data_len - win), win, cudaMemcpyDeviceToDevice, c->stream));
+    // Summary.db is a hint here as everywhere: if its positions do not parse or the slices they give do not tile the call's own
+    // slice, the call runs as one piece (K2 over the whole Index.db)
+    bool cut_pieces(const std::vector<double>& cuts, bool forced_ranges) {
+        const int want_ranges = (int)cuts.size() + 1;
+        int imax = 0; uint64_t nmax = 0;
+        for (int i = 0; i < K; i++) if (isl[i].s_count > nmax) { nmax = isl[i].s_count; imax = i; }
+        if (nmax < (uint64_t)want_ranges * (forced_ranges ? 1 : 32)) return false;
+        const b200c_input& big = m->inputs[imax];
+        std::vector<int64_t> t2{m->token_lo};
+        for (int r = 1; r < want_ranges; r++) {
+            const uint64_t sidx = isl[imax].s_first + std::min<uint64_t>(nmax - 1, (uint64_t)(nmax * cuts[r - 1]));
+            int64_t t = 0;
+            if (!sample_token(big.index, big.index_len, big.summary_positions[sidx], m->partitioner, &t)) return false;
+            if (t > t2.back() && t < m->token_hi) t2.push_back(t);
         }
-    } else {
-        B200C_TRY(ws_typed(c, WS_CD, co + 64, &CD));
-        B200C_TRY(ws_typed(c, WS_CO, oo + 1, &CO));
-        for (int i = 0; i < K; i++) { k1_data[i] = m->inputs[i].compressor == COMP_UNCOMPRESSED ? U + ubase[i] : CD + cbase[i]; k1_offs[i] = CO + obase[i]; }
+        t2.push_back(m->token_hi);
+        const int n2 = (int)t2.size() - 1;
+        if (n2 < 2) return false;
+        std::vector<std::vector<IdxSlice>> p2(n2, isl); std::vector<uint64_t> u2((size_t)n2 * K, 0);
+        for (int r = 0; r < n2; r++) for (int i = 0; i < K; i++) {
+            const b200c_input& in = m->inputs[i];
+            IdxSlice& sl = p2[r][i];
+            if (!in.index_len) { sl = IdxSlice{0, 0, in.data_length, 0, 0}; u2[(size_t)r * K + i] = in.data_length; continue; }
+            if (!compute_index_slice(in.index, in.index_len, in.summary_positions, in.nsummary, in.data_length, m->partitioner, t2[r], t2[r + 1], &sl)) return false;
+            // every entry must lie in some piece's slice: consecutive slices touch or overlap, the first starts and the last ends with the call's own
+            if (r == 0 && sl.lo != isl[i].lo) return false;
+            if (r == n2 - 1 && sl.hi != isl[i].hi) return false;
+            if (r > 0 && (sl.lo > p2[r - 1][i].hi || sl.lo < p2[r - 1][i].lo || sl.hi < p2[r - 1][i].hi)) return false;
+            uint64_t pos = sl.uend;
+            if (sl.hi > sl.lo && !entry_data_position(in.index, in.index_len, sl.lo, in.data_length, &pos)) return false;
+            if (pos > sl.uend) return false;
+            u2[(size_t)r * K + i] = pos;
+        }
+        T = t2; psl = p2; pustart = u2;
+        return true;
     }
-    B200C_TRY(ws_typed(c, WS_IDX, io + 64, &IDX));
-    // Summary.db positions on the device: one run per piece and input (file offsets; K2 subtracts the slice start — no kernel rides on the copy stream)
-    std::vector<std::vector<uint64_t>> psb(nr, std::vector<uint64_t>(K + 1, 0));
-    uint64_t summ_total = 0;
-    for (int r = 0; r < nr; r++) for (int i = 0; i <= K; i++) { psb[r][i] = summ_total; if (i < K) summ_total += psl[r][i].s_count; }
-    uint64_t* d_summ; B200C_TRY(ws_typed(c, WS_SUMM, summ_total + 1, &d_summ));
-    { uint8_t* pp; B200C_TRY(ws_typed(c, WS_PARAMS, sizeof(CParams) + sizeof(InDesc) * (size_t)K, &pp)); dP = (CParams*)pp; hp.in = (const InDesc*)(pp + sizeof(CParams)); }
-    B200C_TRY(ws_typed(c, WS_BBASE, (size_t)K + 1, &d_bbase));
-    { uint8_t* p; B200C_TRY(ws_typed(c, WS_ERR2, 4096, &p)); d_err = (DevErr*)p; d_cerr = (ChunkErr*)(p + 64); d_stats = (RunStats*)(p + 128); d_hist = (unsigned long long*)(p + 256); }
-    hp.U = U;
-    cudaStream_t st = c->stream;
-    if (m->npurge_ranges) {
-        int64_t* d_pt; B200C_TRY(ws_typed(c, WS_PURGE, 2 * (size_t)m->npurge_ranges, &d_pt));
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(d_pt, m->purge_range_hi, 8 * (size_t)m->npurge_ranges, cudaMemcpyHostToDevice, st));
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(d_pt + m->npurge_ranges, m->purge_range_max_ts, 8 * (size_t)m->npurge_ranges, cudaMemcpyHostToDevice, st));
-        hp.purge_hi = d_pt; hp.purge_ts = d_pt + m->npurge_ranges; hp.npurge = m->npurge_ranges;
+
+    // ---- workspace ---------------------------------------------------------------------------------------------------------------------
+    int workspace() {
+        B200C_TRY(ws_typed(c, WS_U, uo + 64, &U));
+        // K1's view of input i. Host inputs are staged in CD / CO (uncompressed ones go to U itself and are verified there). Device-resident inputs are read where the caller keeps them: no copy,
+        // no second image of the compressed inputs in device memory; only the file's tail is staged for the decoders' word reads (k1_src).
+        k1_data.assign(K, nullptr); k1_tail.assign(K, nullptr); k1_offs.assign(K, nullptr); k1_tail_off.assign(K, ~0ull);
+        if (dev) {
+            std::vector<uint64_t> tb(K + 1, 0);
+            // (uncompressed inputs: the ingest kernel reads whole aligned words inside the file only, nothing to stage)
+            auto tail_window = [](const b200c_input& in) -> uint64_t { return in.compressor == COMP_UNCOMPRESSED ? 0 : std::min(in.data_len, k1_tail_window(chunk_max_compressed(in.compressor, in.chunk_len), in.chunk_len)); };
+            for (int i = 0; i < K; i++) tb[i + 1] = tb[i] + ((tail_window(m->inputs[i]) + 64 + 15) & ~15ull);
+            uint8_t* TAIL; B200C_TRY(ws_typed(c, WS_K1TAIL, tb[K] + 64, &TAIL));
+            for (int i = 0; i < K; i++) {
+                const b200c_input& in = m->inputs[i];
+                const uint64_t win = tail_window(in);
+                k1_data[i] = in.data; k1_offs[i] = in.chunk_offsets; k1_tail[i] = TAIL + tb[i]; k1_tail_off[i] = in.data_len - win;
+                if (win) B200C_CUDA_TRY(c, cudaMemcpyAsync(TAIL + tb[i], in.data + (in.data_len - win), win, cudaMemcpyDeviceToDevice, st));
+            }
+        } else {
+            B200C_TRY(ws_typed(c, WS_CD, co + 64, &CD));
+            B200C_TRY(ws_typed(c, WS_CO, oo + 1, &CO));
+            for (int i = 0; i < K; i++) { k1_data[i] = m->inputs[i].compressor == COMP_UNCOMPRESSED ? U + ubase[i] : CD + cbase[i]; k1_offs[i] = CO + obase[i]; }
+        }
+        B200C_TRY(ws_typed(c, WS_IDX, io + 64, &IDX));
+        // Summary.db positions on the device: one run per piece and input (file offsets; K2 subtracts the slice start — no kernel rides on the copy stream)
+        psb.assign(nr, std::vector<uint64_t>(K + 1, 0));
+        uint64_t summ_total = 0;
+        for (int r = 0; r < nr; r++) for (int i = 0; i <= K; i++) { psb[r][i] = summ_total; if (i < K) summ_total += psl[r][i].s_count; }
+        B200C_TRY(ws_typed(c, WS_SUMM, summ_total + 1, &d_summ));
+        { uint8_t* pp; B200C_TRY(ws_typed(c, WS_PARAMS, sizeof(CParams) + sizeof(InDesc) * (size_t)K, &pp)); dP = (CParams*)pp; hp.in = (const InDesc*)(pp + sizeof(CParams)); }
+        B200C_TRY(ws_typed(c, WS_BBASE, (size_t)K + 1, &d_bbase));
+        { uint8_t* p; B200C_TRY(ws_typed(c, WS_ERR2, 4096, &p)); d_err = (DevErr*)p; d_cerr = (ChunkErr*)(p + 64); d_stats = (RunStats*)(p + 128); d_hist = (unsigned long long*)(p + 256); }
+        d_rbytes = (unsigned long long*)(d_stats + 1) + 1;      // (zeroed with the stats block; every K2 run adds its range)
+        hp.U = U;
+        if (m->npurge_ranges) {
+            int64_t* d_pt; B200C_TRY(ws_typed(c, WS_PURGE, 2 * (size_t)m->npurge_ranges, &d_pt));
+            B200C_CUDA_TRY(c, cudaMemcpyAsync(d_pt, m->purge_range_hi, 8 * (size_t)m->npurge_ranges, cudaMemcpyHostToDevice, st));
+            B200C_CUDA_TRY(c, cudaMemcpyAsync(d_pt + m->npurge_ranges, m->purge_range_max_ts, 8 * (size_t)m->npurge_ranges, cudaMemcpyHostToDevice, st));
+            hp.purge_hi = d_pt; hp.purge_ts = d_pt + m->npurge_ranges; hp.npurge = m->npurge_ranges;
+        }
+        meta_interval = m->min_index_interval > 0 ? (uint32_t)m->min_index_interval : 128u;
+        bloom_words = (want_meta && res->outputs[0].filter) ? m->bloom_words : 0;
+        if (want_meta) {
+            B200C_TRY(ws_typed(c, WS_META_SG, 1, &d_sg));
+            B200C_TRY(ws_typed(c, WS_META_TD, 1, &d_td));
+            B200C_TRY(ws_typed(c, WS_META_BLOOM, bloom_words * 2 + 16, &d_bloom));
+            B200C_TRY(ws_typed(c, WS_META_KEYS, (size_t)2 * 65536, &d_mkeys));
+            std::vector<uint8_t> init(sizeof(StatGlobal), 0); StatGlobal* g0 = (StatGlobal*)init.data();
+            g0->min_ts = I64_MAX; g0->max_ts = I64_MIN; g0->min_ldt = I64_MAX; g0->max_ldt = I64_MIN; g0->min_ttl = INT_MAX; g0->max_ttl = INT_MIN;
+            auto offsets = [](long long* o, int n) { long long last = 1; o[0] = 1; for (int i = 1; i < n; i++) { long long next = llround((double)last * 1.2); if (next == last) next++; o[i] = next; last = next; } };
+            offsets(g0->psize_off, META_PSIZE - 1); offsets(g0->cells_off, META_CELLS - 1);       // EstimatedHistogram.newOffsets (S/utils/EstimatedHistogram.java:91-109)
+            B200C_CUDA_TRY(c, cudaMemcpyAsync(d_sg, init.data(), sizeof(StatGlobal), cudaMemcpyHostToDevice, st));
+            B200C_CUDA_TRY(c, cudaStreamSynchronize(st));                                            // (init is a stack vector)
+            B200C_CUDA_TRY(c, cudaMemsetAsync(d_td, 0, sizeof(TdropTable), st));
+            B200C_CUDA_TRY(c, cudaMemsetAsync(d_td->key, 0xFF, sizeof(d_td->key), st));
+            if (bloom_words) B200C_CUDA_TRY(c, cudaMemsetAsync(d_bloom, 0, bloom_words * 8, st));
+        }
+        B200C_CUDA_TRY(c, cudaMemsetAsync(d_err, 0xFF, 64, st));
+        B200C_CUDA_TRY(c, cudaMemsetAsync(d_cerr, 0xFF, 64, st));
+        B200C_CUDA_TRY(c, cudaMemsetAsync(d_stats, 0, 128 + MAXK * 8 + 128, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync((void*)hp.in, hin.data(), sizeof(InDesc) * (size_t)K, cudaMemcpyHostToDevice, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(dP, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(d_bbase, bbase.data(), (K + 1) * 8, cudaMemcpyHostToDevice, st));
+        return B200C_OK;
     }
-    // metadata state (meta.cuh), device resident across the pieces of the call
-    StatGlobal* d_sg = nullptr; TdropTable* d_td = nullptr; uint32_t* d_bloom = nullptr; uint8_t* d_mkeys = nullptr;
-    uint64_t written_total = 0, samples_total = 0; uint8_t* d_sument = nullptr; uint64_t* d_sumoff = nullptr; uint64_t sument_bound = 0;
-    const uint32_t meta_interval = m->min_index_interval > 0 ? (uint32_t)m->min_index_interval : 128u;
-    const uint64_t bloom_words = (want_meta && o0.filter) ? m->bloom_words : 0;
-    if (want_meta) {
-        B200C_TRY(ws_typed(c, WS_META_SG, 1, &d_sg));
-        B200C_TRY(ws_typed(c, WS_META_TD, 1, &d_td));
-        B200C_TRY(ws_typed(c, WS_META_BLOOM, bloom_words * 2 + 16, &d_bloom));
-        B200C_TRY(ws_typed(c, WS_META_KEYS, (size_t)2 * 65536, &d_mkeys));
-        std::vector<uint8_t> init(sizeof(StatGlobal), 0); StatGlobal* g0 = (StatGlobal*)init.data();
-        g0->min_ts = I64_MAX; g0->max_ts = I64_MIN; g0->min_ldt = I64_MAX; g0->max_ldt = I64_MIN; g0->min_ttl = INT_MAX; g0->max_ttl = INT_MIN;
-        auto offsets = [](long long* o, int n) { long long last = 1; o[0] = 1; for (int i = 1; i < n; i++) { long long next = llround((double)last * 1.2); if (next == last) next++; o[i] = next; last = next; } };
-        offsets(g0->psize_off, META_PSIZE - 1); offsets(g0->cells_off, META_CELLS - 1);       // EstimatedHistogram.newOffsets (S/utils/EstimatedHistogram.java:91-109)
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(d_sg, init.data(), sizeof(StatGlobal), cudaMemcpyHostToDevice, st));
-        B200C_CUDA_TRY(c, cudaStreamSynchronize(st));                                            // (init is a stack vector)
-        B200C_CUDA_TRY(c, cudaMemsetAsync(d_td, 0, sizeof(TdropTable), st));
-        B200C_CUDA_TRY(c, cudaMemsetAsync(d_td->key, 0xFF, sizeof(d_td->key), st));
-        if (bloom_words) B200C_CUDA_TRY(c, cudaMemsetAsync(d_bloom, 0, bloom_words * 8, st));
-    }
-    B200C_CUDA_TRY(c, cudaMemsetAsync(d_err, 0xFF, 64, st));
-    B200C_CUDA_TRY(c, cudaMemsetAsync(d_cerr, 0xFF, 64, st));
-    B200C_CUDA_TRY(c, cudaMemsetAsync(d_stats, 0, 128 + MAXK * 8 + 128, st));
-    B200C_CUDA_TRY(c, cudaMemcpyAsync((void*)hp.in, hin.data(), sizeof(InDesc) * (size_t)K, cudaMemcpyHostToDevice, st));
-    B200C_CUDA_TRY(c, cudaMemcpyAsync(dP, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
-    B200C_CUDA_TRY(c, cudaMemcpyAsync(d_bbase, bbase.data(), (K + 1) * 8, cudaMemcpyHostToDevice, st));
-    cudaMemcpyKind kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    uint64_t bytes_read = 0;
-    // inputs are staged on a second stream, one event per input, so that the kernels of input i overlap the copy of input i+1
-    // (the workspace was possibly re-allocated above: make sure that is ordered before the copies)
-    cudaStream_t cs = c->copy_stream;
-    B200C_CUDA_TRY(c, cudaEventRecord(c->ev0, st));
-    B200C_CUDA_TRY(c, cudaStreamWaitEvent(cs, c->ev0, 0));
-    std::vector<uint64_t> h2d_next(K, 0), k1_next(K, 0);      // deferred mode: first chunk of input i not yet copied / not yet decompressed
-    // device-resident inputs taking the piece route (a token sub-range): the host schedules the chunk-range copies, so it needs the offsets too
-    std::vector<std::vector<uint64_t>> co_host(dev && deferred ? K : 0);
-    for (size_t i = 0; i < co_host.size(); i++) {
-        co_host[i].resize(m->inputs[i].nchunks);
-        if (m->inputs[i].nchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(co_host[i].data(), m->inputs[i].chunk_offsets, m->inputs[i].nchunks * 8, cudaMemcpyDeviceToHost, cs));
-    }
-    if (!co_host.empty()) B200C_CUDA_TRY(c, cudaStreamSynchronize(cs));
+
+    // ---- input copies -------------------------------------------------------------------------------------------------------------------
     // file offset of chunk ch of input i (an uncompressed input's chunk i sits at i * chunk_len; its chunk table holds CRCs)
-    auto chunk_off = [&](int i, uint64_t ch) -> uint64_t {
+    uint64_t chunk_off(int i, uint64_t ch) const {
         const b200c_input& in = m->inputs[i];
         if (ch >= in.nchunks) return in.data_len;
         if (in.compressor == COMP_UNCOMPRESSED) return ch * (uint64_t)in.chunk_len;
         return co_host.empty() ? in.chunk_offsets[ch] : co_host[i][ch];
-    };
-    auto copy_chunks = [&](int i, uint64_t a, uint64_t b) -> int {      // compressed bytes of chunks [a, b) of input i -> CD (host inputs; uncompressed -> U)
+    }
+    int copy_chunks(int i, uint64_t a, uint64_t b) {      // compressed bytes of chunks [a, b) of input i -> CD (host inputs; uncompressed -> U)
         const b200c_input& in = m->inputs[i];
         if (a >= b || dev) return B200C_OK;
-        uint64_t lo = chunk_off(i, a), hi = chunk_off(i, b);
-        if (lo > hi || hi > in.data_len) { c->err = "chunk offsets of input " + std::to_string(i) + " are not increasing"; res->corruption.input = i; res->corruption.kind = 2; res->corruption.chunk = a; res->corruption.offset = 0; return B200C_ECORRUPT; }
+        const uint64_t lo = chunk_off(i, a), hi = chunk_off(i, b);
+        if (lo > hi || hi > in.data_len) return corrupt(i, 2, a, 0, "chunk offsets of input " + std::to_string(i) + " are not increasing");
         uint8_t* const to = in.compressor == COMP_UNCOMPRESSED ? U + ubase[i] : CD + cbase[i];
-        if (hi > lo) B200C_CUDA_TRY(c, cudaMemcpyAsync(to + lo, in.data + lo, hi - lo, kind, cs));
+        if (hi > lo) B200C_CUDA_TRY(c, cudaMemcpyAsync(to + lo, in.data + lo, hi - lo, in_kind, cs));
         return B200C_OK;
-    };
-    // what each piece needs from each input: chunks to copy (deferred mode) and to decompress
-    struct Need { uint64_t h2d_a, h2d_b, k1_a, k1_b; };
-    std::vector<Need> need((size_t)nr * K, Need{0, 0, 0, 0});
-    std::vector<uint64_t> range_bytes(nr, 0);
-    std::vector<uint64_t> range_end((size_t)nr * K, 0);          // per piece and input: Data.db position behind the piece (scanner accounting)
-    for (int i = 0; i < K; i++) { bytes_read += m->inputs[i].data_length; range_end[(size_t)(nr - 1) * K + i] = m->inputs[i].data_length; }
-    for (int r = 0; r < nr; r++) range_bytes[r] = bytes_read;
-    auto need_of = [&](int r, int i, uint64_t a, uint64_t b) {      // piece r reads bytes [a, b) of input i's decompressed stream
+    }
+    void need_of(int r, int i, uint64_t a, uint64_t b) {      // piece r reads bytes [a, b) of input i's decompressed stream
         const b200c_input& in = m->inputs[i];
         range_end[(size_t)r * K + i] = b;
         Need& nd = need[(size_t)r * K + i];
@@ -1291,20 +1387,34 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
             nd.h2d_a = std::max(ca, h2d_next[i]); nd.h2d_b = std::max(cb, nd.h2d_a); h2d_next[i] = nd.h2d_b;
             nd.k1_a = std::max(ca, k1_next[i]); nd.k1_b = std::max(cb, nd.k1_a); k1_next[i] = nd.k1_b;
         }
-    };
-    for (int i = 0; i < K; i++) {
-        const b200c_input& in = m->inputs[i];
-        if (!dev && !deferred && in.data_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(in.compressor == COMP_UNCOMPRESSED ? U + ubase[i] : CD + cbase[i], in.data, in.data_len, kind, cs));
-        if (!dev && in.nchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(CO + obase[i], in.chunk_offsets, in.nchunks * 8, kind, cs));
-        if (!istream) {
-            if (isl[i].hi > isl[i].lo) B200C_CUDA_TRY(c, cudaMemcpyAsync(IDX + ibase[i], in.index + isl[i].lo, isl[i].hi - isl[i].lo, kind, cs));
-            if (isl[i].s_count) {
-                B200C_CUDA_TRY(c, cudaMemcpyAsync(d_summ + psb[0][i], in.summary_positions + isl[i].s_first, isl[i].s_count * 8, kind, cs));
-            }
-        }
-        B200C_CUDA_TRY(c, cudaEventRecord(c->ev_in[i], cs));
     }
-    if (istream) {
+    // inputs are staged on the copy stream, one event per input, so that the kernels of input i overlap the copy of input i+1
+    int stage_inputs() {
+        // (the workspace was possibly re-allocated above: make sure that is ordered before the copies)
+        B200C_CUDA_TRY(c, cudaEventRecord(c->ev0, st));
+        B200C_CUDA_TRY(c, cudaStreamWaitEvent(cs, c->ev0, 0));
+        h2d_next.assign(K, 0); k1_next.assign(K, 0);
+        // device-resident inputs taking the piece route (a token sub-range): the host schedules the chunk-range copies, so it needs the offsets too
+        co_host.resize(dev && deferred ? K : 0);
+        for (size_t i = 0; i < co_host.size(); i++) {
+            co_host[i].resize(m->inputs[i].nchunks);
+            if (m->inputs[i].nchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(co_host[i].data(), m->inputs[i].chunk_offsets, m->inputs[i].nchunks * 8, cudaMemcpyDeviceToHost, cs));
+        }
+        if (!co_host.empty()) B200C_CUDA_TRY(c, cudaStreamSynchronize(cs));
+        need.assign((size_t)nr * K, Need{0, 0, 0, 0}); range_end.assign((size_t)nr * K, 0);
+        for (int i = 0; i < K; i++) { bytes_read += m->inputs[i].data_length; range_end[(size_t)(nr - 1) * K + i] = m->inputs[i].data_length; }
+        range_bytes.assign(nr, bytes_read);
+        for (int i = 0; i < K; i++) {
+            const b200c_input& in = m->inputs[i];
+            if (!dev && !deferred && in.data_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(in.compressor == COMP_UNCOMPRESSED ? U + ubase[i] : CD + cbase[i], in.data, in.data_len, in_kind, cs));
+            if (!dev && in.nchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(CO + obase[i], in.chunk_offsets, in.nchunks * 8, in_kind, cs));
+            if (!istream) {
+                if (isl[i].hi > isl[i].lo) B200C_CUDA_TRY(c, cudaMemcpyAsync(IDX + ibase[i], in.index + isl[i].lo, isl[i].hi - isl[i].lo, in_kind, cs));
+                if (isl[i].s_count) B200C_CUDA_TRY(c, cudaMemcpyAsync(d_summ + psb[0][i], in.summary_positions + isl[i].s_first, isl[i].s_count * 8, in_kind, cs));
+            }
+            B200C_CUDA_TRY(c, cudaEventRecord(c->ev_in[i], cs));
+        }
+        if (!istream) return B200C_OK;
         // piece after piece: the Index.db bytes not copied yet (consecutive slices overlap by a sample interval), the piece's Summary positions,
         // its Data.db chunks; EV_RANGE + r fires when piece r is on the device
         std::vector<uint64_t> idx_copied(K);
@@ -1314,10 +1424,8 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
             for (int i = 0; i < K; i++) {
                 const b200c_input& in = m->inputs[i]; const IdxSlice& sl = psl[r][i];
                 const uint64_t from = std::max(sl.lo, idx_copied[i]);
-                if (sl.hi > from) { B200C_CUDA_TRY(c, cudaMemcpyAsync(IDX + ibase[i] + (from - isl[i].lo), in.index + from, sl.hi - from, kind, cs)); idx_copied[i] = sl.hi; }
-                if (sl.s_count) {
-                    B200C_CUDA_TRY(c, cudaMemcpyAsync(d_summ + psb[r][i], in.summary_positions + sl.s_first, sl.s_count * 8, kind, cs));
-                }
+                if (sl.hi > from) { B200C_CUDA_TRY(c, cudaMemcpyAsync(IDX + ibase[i] + (from - isl[i].lo), in.index + from, sl.hi - from, in_kind, cs)); idx_copied[i] = sl.hi; }
+                if (sl.s_count) B200C_CUDA_TRY(c, cudaMemcpyAsync(d_summ + psb[r][i], in.summary_positions + sl.s_first, sl.s_count * 8, in_kind, cs));
                 need_of(r, i, pustart[(size_t)r * K + i], sl.uend);
                 tot += sl.uend - pustart[(size_t)r * K + i];
                 B200C_TRY(copy_chunks(i, need[(size_t)r * K + i].h2d_a, need[(size_t)r * K + i].h2d_b));
@@ -1325,33 +1433,11 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
             range_bytes[r] = tot;
             B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_RANGE + r], cs));
         }
+        return B200C_OK;
     }
-    c->prog_total.store(bytes_read); c->prog_scanned.store(0);
-    for (int i = 0; i < K; i++) c->prog_input_pos[i].store(0);
-    c->prog_ninputs.store(K);
-    timing_begin(c);
 
-    // stage clock: marks on the main stream; the time between two marks is charged to the stage of the first
-    struct Mark { int stage; cudaEvent_t ev; };
-    std::vector<Mark> marks;
-    size_t k5_marks = 0;
-    auto mark = [&](int stage) {
-        size_t k = marks.size();
-        if (k >= c->ev_marks.size()) { cudaEvent_t e; cudaEventCreate(&e); c->ev_marks.push_back(e); }
-        cudaEventRecord(c->ev_marks[k], st); marks.push_back(Mark{stage, c->ev_marks[k]});
-    };
-    auto finish_marks = [&]() {
-        for (int k = 0; k < 8; k++) c->stage_ms[k] = 0;
-        for (size_t k = 0; k + 1 < marks.size(); k++) { float ms = 0; cudaEventElapsedTime(&ms, marks[k].ev, marks[k + 1].ev); if (marks[k].stage >= 0) c->stage_ms[marks[k].stage] += ms; }
-        for (size_t k = 0; k + 1 < k5_marks; k += 2) { float ms = 0; if (cudaEventElapsedTime(&ms, c->ev_k5[k], c->ev_k5[k + 1]) == cudaSuccess) c->stage_ms[5] += ms; }      // K5 on stream5: overlaps the next piece's stages
-        c->nstages = 6;
-    };
-    c->nstages = 0;
-    mark(0);
-
-    // ---- K1: decompress + verify (deferred mode: K1 runs per token range further down) ---------------------------------------------------
-    c->prog_stage.store(1);
-    auto k1 = [&](int i, uint64_t a, uint64_t b) -> int {           // chunks [a, b) of input i
+    // ---- K1: decompress + verify (deferred mode: K1 runs per token range, in piece()) ---------------------------------------------------
+    int k1(int i, uint64_t a, uint64_t b) {           // chunks [a, b) of input i
         const b200c_input& in = m->inputs[i];
         if (a >= b) return B200C_OK;
         if (in.compressor == COMP_UNCOMPRESSED) {          // verify against CRC.db; device-resident inputs are copied into U on the way
@@ -1362,14 +1448,11 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         }
         return decompress_stream_device(c, in.compressor, k1_data[i], in.data_len, k1_offs[i], in.nchunks, in.chunk_len,
                                         in.max_compressed_len, in.data_length, U + ubase[i], 1, d_cerr, a, b - a, i, k1_tail[i], k1_tail_off[i]);
-    };
+    }
     // several inputs' chunk ranges in one thread-per-chunk launch when there are enough of them (B200C_K1_BATCH=0 switches it off)
-    const int k1_batch_env = []() { const char* e = getenv("B200C_K1_BATCH"); return e ? atoi(e) : (B200C_K1_BATCH_DEFAULT ? 1 : 0); }();     // 2: batch even tiny launches (tests)
-    const bool k1_batching = k1_batch_env != 0;
-    std::vector<K1Seg> segs; segs.reserve(K);
-    auto k1_many = [&](const std::vector<uint64_t>& from, const std::vector<uint64_t>& to) -> int {      // chunks [from[i], to[i]) of every input
+    int k1_many(const std::vector<uint64_t>& from, const std::vector<uint64_t>& to) {      // chunks [from[i], to[i]) of every input
         segs.clear(); uint64_t total = 0;
-        for (int i = 0; i < K && k1_batching; i++) {
+        for (int i = 0; i < K && k1_batch_env != 0; i++) {
             const b200c_input& in = m->inputs[i];
             if (from[i] >= to[i] || in.compressor != COMP_LZ4 || (in.chunk_len & 7)) continue;
             K1Seg g; memset(&g, 0, sizeof(g));
@@ -1387,48 +1470,46 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
             B200C_TRY(k1(i, from[i], to[i]));
         }
         return B200C_OK;
-    };
-    // K1 waits for what it reads: host inputs' chunk offsets and (unless the pieces bring their own) Data.db. Device-resident inputs are
-    // read in place; their Index.db / Summary.db staging runs under K1 and K2 waits for it.
-    auto wait_inputs = [&]() -> int { for (int i = 0; i < K; i++) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_in[i], 0)); return B200C_OK; };
-    if (!dev) B200C_TRY(wait_inputs());
-    if (!deferred) {
-        if (dev && k1_batching) {          // device-resident inputs: decode in one launch
+    }
+    int wait_inputs() { for (int i = 0; i < K; i++) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_in[i], 0)); return B200C_OK; }
+    // the stage clock starts; K1 over whole inputs unless the pieces decode their own chunks
+    int k1_inputs() {
+        c->prog_total.store(bytes_read); c->prog_scanned.store(0);
+        for (int i = 0; i < K; i++) c->prog_input_pos[i].store(0);
+        c->prog_ninputs.store(K);
+        timing_begin(c);
+        c->nstages = 0;
+        mark(0);
+        c->prog_stage.store(1);
+        k1_batch_env = []() { const char* e = getenv("B200C_K1_BATCH"); return e ? atoi(e) : (B200C_K1_BATCH_DEFAULT ? 1 : 0); }();     // 2: batch even tiny launches (tests)
+        // K1 waits for what it reads: host inputs' chunk offsets and (unless the pieces bring their own) Data.db. Device-resident inputs are
+        // read in place; their Index.db / Summary.db staging runs under K1 and K2 waits for it.
+        if (!dev) B200C_TRY(wait_inputs());
+        if (deferred) return B200C_OK;
+        if (dev && k1_batch_env != 0) {          // device-resident inputs: decode in one launch
             std::vector<uint64_t> z(K, 0), e(K);
             for (int i = 0; i < K; i++) e[i] = m->inputs[i].nchunks;
-            B200C_TRY(k1_many(z, e));
-        } else for (int i = 0; i < K; i++) B200C_TRY(k1(i, 0, m->inputs[i].nchunks));
+            return k1_many(z, e);
+        }
+        for (int i = 0; i < K; i++) B200C_TRY(k1(i, 0, m->inputs[i].nchunks));
+        return B200C_OK;
     }
-    uint64_t* h = (uint64_t*)c->h_pinned;
-    // the request is consumed by the call that reports it (b200c.h: sticky until then, so one that lands before the call is not lost)
-    auto check_cancel = [&]() -> int { if (c->cancel.exchange(0)) { c->err = "cancelled"; cudaStreamSynchronize(st); timing_end(c); return B200C_ECANCELLED; } return B200C_OK; };
-    auto chunk_error = [&](uint64_t word) -> int {                  // word = d_cerr: (input << 48 | chunk << 8 | kind)
-        int which = (int)(word >> 48), kindc = (int)(word & 0xff); uint64_t chunk = (word >> 8) & 0xFFFFFFFFFFull;
-        // an uncompressed input's chunk starts at chunk * chunk_len of Data.db
-        const uint64_t off = which < K && m->inputs[which].compressor == COMP_UNCOMPRESSED ? chunk * (uint64_t)m->inputs[which].chunk_len : 0;
-        res->corruption.input = which; res->corruption.kind = kindc; res->corruption.chunk = chunk; res->corruption.offset = off;
-        c->err = std::string(kindc == 1 ? "chunk CRC mismatch" : "malformed compressed chunk") + " in input " + std::to_string(which) + " chunk " + std::to_string(chunk);
-        timing_end(c);
-        return B200C_ECORRUPT;
-    };
-    auto index_data_mismatch = [&](uint64_t word) -> int {
-        res->corruption.input = (int)((word >> 48) & 0xFF); res->corruption.kind = 3; res->corruption.chunk = 0; res->corruption.offset = word & 0xFFFFFFFFFFFFull;
-        c->err = "Index.db does not match Data.db in input " + std::to_string(res->corruption.input);
-        timing_end(c);
-        return B200C_ECORRUPT;
-    };
 
-    // ---- K2: Index.db -> tokens, key prefixes, positions of the partitions the slices `sl` describe (speculate from the Summary.db samples,
-    //      prove against the sequential parse, emit), order check, and the partitions of every input inside (tlo, thi] ---------------------
-    uint64_t total_parts = 0;
-    std::vector<uint64_t> pcount(K, 0), pbase(K + 1, 0);
-    int64_t* d_tok = nullptr; uint64_t *d_kp = nullptr, *d_upos = nullptr, *d_pbase = nullptr, *d_pcount = nullptr, *d_range = nullptr; uint16_t* d_klen = nullptr;
-    B200C_TRY(ws_typed(c, WS_PBASE, (size_t)2 * K + 2, &d_pbase)); d_pcount = d_pbase + K + 1;
-    B200C_TRY(ws_typed(c, WS_RANGE, (size_t)2 * K + 16, &d_range));
-    unsigned long long* d_rbytes = (unsigned long long*)(d_stats + 1) + 1;      // (zeroed with the stats block; every K2 run adds its range)
-    res->index_slow_path_inputs = 0;
-    uint64_t slow_inputs = 0;
-    auto k2_run = [&](const std::vector<IdxSlice>& sl, const std::vector<uint64_t>& sb, int64_t tlo, int64_t thi) -> int {
+    // ---- K2: Index.db -> tokens, key prefixes, positions of the partitions the slices `sl` describe, order check, and the partitions of
+    //      every input inside (tlo, thi] ------------------------------------------------------------------------------------------------
+    // K2 over the call's slices unless the pieces bring their own, then the plan of a single deferred piece
+    int k2_inputs() {
+        pcount.assign(K, 0); pbase.assign(K + 1, 0);
+        B200C_TRY(ws_typed(c, WS_PBASE, (size_t)2 * K + 2, &d_pbase)); d_pcount = d_pbase + K + 1;
+        B200C_TRY(ws_typed(c, WS_RANGE, (size_t)2 * K + 16, &d_range));
+        res->index_slow_path_inputs = 0;
+        mark(1);
+        if (dev) B200C_TRY(wait_inputs());
+        if (!istream) B200C_TRY(k2(isl, psb[0], m->token_lo, m->token_hi));
+        if (deferred && !istream) B200C_TRY(plan_chunks());
+        return B200C_OK;
+    }
+    int k2(const std::vector<IdxSlice>& sl, const std::vector<uint64_t>& sb, int64_t tlo, int64_t thi) {
         c->prog_stage.store(2);
         uint64_t bo2 = 0;
         for (int i = 0; i < K; i++) {
@@ -1437,61 +1518,72 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
             hin[i].ibase = ibase[i] + (sl[i].lo - isl[i].lo); hin[i].ilen = ilen_i; hin[i].uend = sl[i].uend;
         }
         bbase[K] = bo2;
-        const uint64_t nblocks = bo2;
         B200C_CUDA_TRY(c, cudaMemcpyAsync((void*)hp.in, hin.data(), sizeof(InDesc) * (size_t)K, cudaMemcpyHostToDevice, st));
         B200C_CUDA_TRY(c, cudaMemcpyAsync(d_bbase, bbase.data(), (K + 1) * 8, cudaMemcpyHostToDevice, st));
-        auto alloc_arrays = [&]() -> int {
-            B200C_TRY(check_cancel());
-            if (total_parts - K >= (1ull << 40)) { c->err = "too many partitions"; return B200C_EUNSUPPORTED; }
-            B200C_TRY(ws_typed(c, WS_TOK, total_parts + 1, &d_tok));
-            B200C_TRY(ws_typed(c, WS_KP, total_parts + 1, &d_kp));
-            B200C_TRY(ws_typed(c, WS_KLEN, total_parts + 1, &d_klen));
-            B200C_TRY(ws_typed(c, WS_UPOS, total_parts + 1, &d_upos));
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(d_pbase, pbase.data(), (K + 1) * 8, cudaMemcpyHostToDevice, st));
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(d_pcount, pcount.data(), K * 8, cudaMemcpyHostToDevice, st));
-            return B200C_OK;
-        };
-        // ---- with Summary.db samples: one thread per Summary interval of every input, count + prove, scan, emit + order check (k_index_walk_*).
-        //      B200C_K2_LEGACY=1 (A/B) runs the speculate-chain-verify path below instead, which also serves inputs without samples, samples
-        //      sparser than 64 KiB per interval (one thread's serial walk would be too long) and any input whose samples did not prove.
-        //      (B200C_K2_INTERVALS=1, which selected the walk by interval while it was not the default, is accepted and changes nothing.)
-        bool emitted = false;
-        const bool k2_legacy = getenv("B200C_K2_LEGACY") != nullptr;
-        bool intervals_ok = have_summaries && !k2_legacy;
-        for (int i = 0; i < K && intervals_ok; i++)
-            if (sl[i].hi > sl[i].lo && (!sl[i].s_count || (sl[i].hi - sl[i].lo) / sl[i].s_count > (64u << 10))) intervals_ok = false;
-        if (intervals_ok) {
-            K2Walk W; memset(&W, 0, sizeof(W));
-            W.ninputs = K;
-            for (int i = 0; i < K; i++) { W.abase[i + 1] = W.abase[i] + sl[i].s_count; W.sbase[i] = sb[i]; W.bias[i] = sl[i].lo; }
-            const uint64_t na = W.abase[K];
-            uint32_t *d_acnt, *d_abad; uint64_t* d_ascan;
-            B200C_TRY(ws_typed(c, WS_ICNT, na + 1, &d_acnt));
-            B200C_TRY(ws_typed(c, WS_ISCAN, na + 2, &d_ascan));
-            B200C_TRY(ws_typed(c, WS_IBAD, (size_t)K + 1, &d_abad));
-            B200C_CUDA_TRY(c, cudaMemsetAsync(d_abad, 0, (K + 1) * 4, st));
-            const unsigned grid = (unsigned)((na + EW_THREADS - 1) / EW_THREADS);
-            if (na) {
-                B200C_LAUNCH(c, k_index_walk_count, grid, EW_THREADS, 0, dP, IDX, d_summ, W, na, d_acnt, d_abad);
-                B200C_TRY(exclusive_scan<uint32_t>(c, d_acnt, na, d_ascan, WS_SCANA, 0));
-            } else B200C_CUDA_TRY(c, cudaMemsetAsync(d_ascan, 0, 16, st));
-            for (int i = 0; i <= K; i++) B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 8 + i, d_ascan + W.abase[i], 8, cudaMemcpyDeviceToHost, st));
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_cerr, 8, cudaMemcpyDeviceToHost, st));
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 300, d_abad, (K + 1) * 4, cudaMemcpyDeviceToHost, st));
-            B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-            if (h[0] != ~0ull) return chunk_error(h[0]);
-            bool any_bad = false;
-            for (int i = 0; i < K; i++) if (((uint32_t*)(h + 300))[i]) any_bad = true;
-            if (!any_bad) {
-                total_parts = 0;
-                for (int i = 0; i < K; i++) { pcount[i] = h[8 + i + 1] - h[8 + i]; pbase[i] = total_parts; total_parts += pcount[i] + 1; }
-                pbase[K] = total_parts;
-                B200C_TRY(alloc_arrays());
-                if (na) B200C_LAUNCH(c, k_index_walk_emit, grid, EW_THREADS, 0, dP, IDX, d_summ, W, na, d_ascan, d_pbase, d_tok, d_kp, d_klen, d_upos, d_err);
-                emitted = true;
-            }
-        }
-        if (!emitted) {
+        // with Summary.db samples: the walk by interval. B200C_K2_LEGACY=1 (A/B) runs the speculate-chain-verify path instead, which also
+        // serves inputs without samples, samples sparser than 64 KiB per interval (one thread's serial walk would be too long) and any input
+        // whose samples did not prove.
+        bool walk = have_summaries && getenv("B200C_K2_LEGACY") == nullptr, emitted = false;
+        for (int i = 0; i < K && walk; i++)
+            if (sl[i].hi > sl[i].lo && (!sl[i].s_count || (sl[i].hi - sl[i].lo) / sl[i].s_count > (64u << 10))) walk = false;
+        if (walk) B200C_TRY(k2_walk(sl, sb, emitted));
+        if (!emitted) B200C_TRY(k2_speculate(sl, sb, bo2));
+        B200C_LAUNCH(c, k_input_ranges, (K + 63) / 64, 64, 0, dP, d_pbase, d_pcount, d_tok, d_upos, tlo, thi, d_range, d_rbytes);
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(P->range, d_range, 2 * K * 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->err, d_err, 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
+        if (P->err != ~0ull) return index_data_mismatch(P->err);
+        for (int i = 0; i < K; i++) if (P->range[2 * i] > P->range[2 * i + 1] || P->range[2 * i + 1] > pcount[i]) return index_data_mismatch((uint64_t)i << 48);
+        // a slice that does not start with the call's own slice starts at a sample at or below tlo: its first entry is not in range. One that
+        // is — the Summary.db positions lied about the tokens — could hide partitions of this range in the previous slice: refuse it.
+        for (int i = 0; i < K; i++) if (pcount[i] && sl[i].lo != isl[i].lo && P->range[2 * i] == 0) return corrupt(i, 3, 0, sl[i].lo, "Summary.db positions of input " + std::to_string(i) + " do not bracket the token range");
+        return B200C_OK;
+    }
+    // per-input partition counts (P->scan) -> pbase, and the per-partition arrays
+    int partitions() {
+        total_parts = 0;
+        for (int i = 0; i < K; i++) { pcount[i] = P->scan[i + 1] - P->scan[i]; pbase[i] = total_parts; total_parts += pcount[i] + 1; }
+        pbase[K] = total_parts;
+        B200C_TRY(check_cancel());
+        if (total_parts - K >= (1ull << 40)) { c->err = "too many partitions"; return B200C_EUNSUPPORTED; }
+        B200C_TRY(ws_typed(c, WS_TOK, total_parts + 1, &d_tok));
+        B200C_TRY(ws_typed(c, WS_KP, total_parts + 1, &d_kp));
+        B200C_TRY(ws_typed(c, WS_KLEN, total_parts + 1, &d_klen));
+        B200C_TRY(ws_typed(c, WS_UPOS, total_parts + 1, &d_upos));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(d_pbase, pbase.data(), (K + 1) * 8, cudaMemcpyHostToDevice, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(d_pcount, pcount.data(), K * 8, cudaMemcpyHostToDevice, st));
+        return B200C_OK;
+    }
+    // one thread per Summary interval of every input: count + prove, scan, emit + order check (k_index_walk_*). emitted = false: some
+    // interval did not prove, the speculating path takes over
+    int k2_walk(const std::vector<IdxSlice>& sl, const std::vector<uint64_t>& sb, bool& emitted) {
+        K2Walk W; memset(&W, 0, sizeof(W));
+        W.ninputs = K;
+        for (int i = 0; i < K; i++) { W.abase[i + 1] = W.abase[i] + sl[i].s_count; W.sbase[i] = sb[i]; W.bias[i] = sl[i].lo; }
+        const uint64_t na = W.abase[K];
+        uint32_t *d_acnt, *d_abad; uint64_t* d_ascan;
+        B200C_TRY(ws_typed(c, WS_ICNT, na + 1, &d_acnt));
+        B200C_TRY(ws_typed(c, WS_ISCAN, na + 2, &d_ascan));
+        B200C_TRY(ws_typed(c, WS_IBAD, (size_t)K + 1, &d_abad));
+        B200C_CUDA_TRY(c, cudaMemsetAsync(d_abad, 0, (K + 1) * 4, st));
+        const unsigned grid = (unsigned)((na + EW_THREADS - 1) / EW_THREADS);
+        if (na) {
+            B200C_LAUNCH(c, k_index_walk_count, grid, EW_THREADS, 0, dP, IDX, d_summ, W, na, d_acnt, d_abad);
+            B200C_TRY(exclusive_scan<uint32_t>(c, d_acnt, na, d_ascan, WS_SCANA, 0));
+        } else B200C_CUDA_TRY(c, cudaMemsetAsync(d_ascan, 0, 16, st));
+        for (int i = 0; i <= K; i++) B200C_CUDA_TRY(c, cudaMemcpyAsync(P->scan + i, d_ascan + W.abase[i], 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->cerr, d_cerr, 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(P->bad, d_abad, (K + 1) * 4, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
+        if (P->cerr != ~0ull) return chunk_error(P->cerr);
+        for (int i = 0; i < K; i++) if (P->bad[i]) return B200C_OK;
+        B200C_TRY(partitions());
+        if (na) B200C_LAUNCH(c, k_index_walk_emit, grid, EW_THREADS, 0, dP, IDX, d_summ, W, na, d_ascan, d_pbase, d_tok, d_kp, d_klen, d_upos, d_err);
+        emitted = true;
+        return B200C_OK;
+    }
+    // speculate from the Summary.db samples (or every 256-byte block), chain, prove against the sequential parse, emit, check the order
+    int k2_speculate(const std::vector<IdxSlice>& sl, const std::vector<uint64_t>& sb, uint64_t nblocks) {
         uint64_t *d_istart, *d_iend, *d_iscan; uint32_t *d_icnt, *d_ihit, *d_ibad;
         B200C_TRY(ws_typed(c, WS_ISTART, nblocks + 1, &d_istart));
         B200C_TRY(ws_typed(c, WS_IEND, nblocks + 1, &d_iend));
@@ -1519,61 +1611,35 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
             B200C_TRY(exclusive_scan<uint32_t>(c, d_icnt, nblocks, d_iscan, WS_SCANA, 0));
         } else B200C_CUDA_TRY(c, cudaMemsetAsync(d_iscan, 0, 16, st));
         // read back: chunk errors, index errors, per-input partition counts
-        for (int i = 0; i <= K; i++) B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 8 + i, d_iscan + bbase[i], 8, cudaMemcpyDeviceToHost, st));
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_cerr, 8, cudaMemcpyDeviceToHost, st));
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 1, d_err, 8, cudaMemcpyDeviceToHost, st));
-        if (nblocks) B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 300, d_ibad, (K + 1) * 4, cudaMemcpyDeviceToHost, st));
+        for (int i = 0; i <= K; i++) B200C_CUDA_TRY(c, cudaMemcpyAsync(P->scan + i, d_iscan + bbase[i], 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->cerr, d_cerr, 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->err, d_err, 8, cudaMemcpyDeviceToHost, st));
+        if (nblocks) B200C_CUDA_TRY(c, cudaMemcpyAsync(P->bad, d_ibad, (K + 1) * 4, cudaMemcpyDeviceToHost, st));
         B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-        if (nblocks) for (int i = 0; i < K && i < 64; i++) if (((uint32_t*)(h + 300))[i]) slow_inputs |= 1ull << i;
+        if (nblocks) for (int i = 0; i < K && i < 64; i++) if (P->bad[i]) slow_inputs |= 1ull << i;
         res->index_slow_path_inputs = __builtin_popcountll(slow_inputs);
-        if (h[0] != ~0ull) return chunk_error(h[0]);
-        if (h[1] != ~0ull) {
-            res->corruption.input = (int)((h[1] >> 48) & 0xFF); res->corruption.kind = (int)(h[1] >> 56); res->corruption.chunk = 0; res->corruption.offset = h[1] & 0xFFFFFFFFFFFFull;
-            c->err = "malformed Index.db in input " + std::to_string(res->corruption.input);
-            timing_end(c);
-            return B200C_ECORRUPT;
-        }
-        total_parts = 0;
-        for (int i = 0; i < K; i++) { pcount[i] = h[8 + i + 1] - h[8 + i]; pbase[i] = total_parts; total_parts += pcount[i] + 1; }
-        pbase[K] = total_parts;
-        B200C_TRY(alloc_arrays());
+        if (P->cerr != ~0ull) return chunk_error(P->cerr);
+        if (P->err != ~0ull) { const int in = (int)((P->err >> 48) & 0xFF); return corrupt(in, (int)(P->err >> 56), 0, P->err & 0xFFFFFFFFFFFFull, "malformed Index.db in input " + std::to_string(in)); }
+        B200C_TRY(partitions());
         if (nblocks) B200C_LAUNCH(c, k_index_emit, (unsigned)((nblocks + 255) / 256), 256, 0, dP, IDX, d_bbase, nblocks, d_istart, d_icnt, d_iscan, d_pbase,
                                   d_tok, d_kp, d_klen, d_upos, d_err);
         if (total_parts > (uint64_t)K) B200C_LAUNCH(c, k_check_order, 8 * c->nsm, 256, 0, dP, d_pbase, d_pcount, d_tok, d_kp, d_klen, d_upos, d_err);
-        }      // (speculate-chain-verify path; the walk by interval checks the order as it emits)
-        B200C_LAUNCH(c, k_input_ranges, (K + 63) / 64, 64, 0, dP, d_pbase, d_pcount, d_tok, d_upos, tlo, thi, d_range, d_rbytes);
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_range, 2 * K * 8, cudaMemcpyDeviceToHost, st));
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 200, d_err, 8, cudaMemcpyDeviceToHost, st));
-        B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-        if (h[200] != ~0ull) return index_data_mismatch(h[200]);
-        for (int i = 0; i < K; i++) if (h[2 * i] > h[2 * i + 1] || h[2 * i + 1] > pcount[i]) return index_data_mismatch((uint64_t)i << 48);
-        // a slice that does not start with the call's own slice starts at a sample at or below tlo: its first entry is not in range. One that
-        // is — the Summary.db positions lied about the tokens — could hide partitions of this range in the previous slice: refuse it.
-        for (int i = 0; i < K; i++) if (pcount[i] && sl[i].lo != isl[i].lo && h[2 * i] == 0) {
-            c->err = "Summary.db positions of input " + std::to_string(i) + " do not bracket the token range"; res->corruption.input = i; res->corruption.kind = 3; res->corruption.chunk = 0; res->corruption.offset = sl[i].lo;
-            timing_end(c); return B200C_ECORRUPT; }
         return B200C_OK;
-    };
-    mark(1);
-    if (dev) B200C_TRY(wait_inputs());
-    if (!istream) B200C_TRY(k2_run(isl, psb[0], m->token_lo, m->token_hi));
-
-    // ---- token ranges: T[0] < T[1] < ... < T[nr]; piece r merges the partitions with token in (T[r], T[r+1]]. Several pieces: planned on the
-    //      host above (Index.db streaming). One piece of a token sub-range over device-resident inputs: the chunks it crosses come from here.
-    if (deferred && !istream) {
+    }
+    // One piece of a token sub-range (a single deferred piece, host or device-resident inputs): the chunks it crosses come from K2's
+    // partitions. T[0] < T[1] < ... < T[nr]; piece r merges the partitions with token in (T[r], T[r+1]].
+    int plan_chunks() {
         int64_t* d_T; uint64_t* d_plan;
         B200C_TRY(ws_typed(c, WS_PLAN, (size_t)nr + 2 + 2 * (size_t)nr * K, &d_T)); d_plan = (uint64_t*)(d_T + nr + 2);
         B200C_CUDA_TRY(c, cudaMemcpyAsync(d_T, T.data(), (nr + 1) * 8, cudaMemcpyHostToDevice, st));
         B200C_LAUNCH(c, k_range_plan, (unsigned)((nr * K + 63) / 64), 64, 0, dP, d_pbase, d_pcount, d_tok, d_upos, d_T, nr, d_plan);
-        uint64_t* hplan = h + 2048;
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(hplan, d_plan, 2 * (size_t)nr * K * 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(P->plan, d_plan, 2 * (size_t)nr * K * 8, cudaMemcpyDeviceToHost, st));
         B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
         for (int r = 0; r < nr; r++) {
             uint64_t tot = 0;
             for (int i = 0; i < K; i++) {
-                const b200c_input& in = m->inputs[i];
-                uint64_t a = hplan[2 * ((size_t)r * K + i)], b = hplan[2 * ((size_t)r * K + i) + 1];
-                if (a < ubase[i] || b < a || b > ubase[i] + in.data_length) return index_data_mismatch(((uint64_t)i << 48));
+                uint64_t a = P->plan[2 * ((size_t)r * K + i)], b = P->plan[2 * ((size_t)r * K + i) + 1];
+                if (a < ubase[i] || b < a || b > ubase[i] + m->inputs[i].data_length) return index_data_mismatch(((uint64_t)i << 48));
                 a -= ubase[i]; b -= ubase[i]; tot += b - a;
                 need_of(r, i, a, b);
             }
@@ -1584,57 +1650,55 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
             for (int i = 0; i < K; i++) B200C_TRY(copy_chunks(i, need[(size_t)r * K + i].h2d_a, need[(size_t)r * K + i].h2d_b));
             B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_RANGE + r], cs));
         }
+        return B200C_OK;
     }
 
-    // ---- per-piece state -------------------------------------------------------------------------------------------------------------
-    const bool to_host_stream = !dev && !lcs;          // one output file in host memory: K5 pieces leave through an OutStream
-    static const bool two_pass = getenv("B200C_K4_TWO_PASS") != nullptr;     // A/B switch: size pass + full emit pass instead of scratch + gather
-    b200c_output& out0 = res->outputs[0];
-    OutStream os;
-    // B200C_K5_OVERLAP=1 (A/B; no gain on an earlier GPU, not re-measured on the H100; K4 and K5 are both bound by shared memory and latency, the
-    // time K5 spends under the next piece's K1..K3 comes back as slower K2..K4): K5 of piece r on its own stream instead of the main one
-    const bool raw_out = m->out_compressor == COMP_UNCOMPRESSED;       // compression disabled: Data.db + CRC.db (k_raw_checksum)
-    const bool k5_async = to_host_stream && nr > 1 && !raw_out && []() { const char* e = getenv("B200C_K5_OVERLAP"); return e ? atoi(e) != 0 : false; }();
-    int k5_last = -1;
-    if (to_host_stream) B200C_TRY(out_stream_begin(os, c, m->out_compressor, m->out_chunk_len, m->out_max_compressed_len, out0.data, out0.data_cap, WS_CODEC));
-    const uint64_t L = (uint64_t)m->out_chunk_len;
-    uint64_t ubase_total = 0, ilen_total = 0, ncontrib_total = 0, nparts_total = 0;
-    uint64_t tail_len = 0; const uint8_t* tail_ptr = nullptr;       // bytes of the merged stream not yet handed to K5 (< one chunk)
-    bool index_fits = true;
-    // arrays that outlive the loop when there is a single piece (the LCS writer below works on them)
-    uint64_t nparts = 0, ulen_out = 0, ilen_out = 0;
-    uint64_t *d_dsize = nullptr, *d_dpos = nullptr, *d_ipos = nullptr, *d_contrib = nullptr, *d_opfirst = nullptr, *d_ioff = nullptr; uint32_t *d_ipay = nullptr, *d_nblk = nullptr, *d_ihead = nullptr, *d_isize = nullptr, *d_icap = nullptr;
-    uint32_t *d_stmunf = nullptr, *d_strows = nullptr; uint8_t* d_ovf = nullptr;
-    uint8_t *UOUT = nullptr, *IOUT = nullptr, *ISCR = nullptr;
-    K4Args ka; memset(&ka, 0, sizeof(ka));
-    std::function<int(int)> launch_k4;
-
-    for (int r = 0; r < nr; r++) {
+    // ---- the pieces ------------------------------------------------------------------------------------------------------------------
+    int begin_output() {
+        static const bool two_pass_env = getenv("B200C_K4_TWO_PASS") != nullptr;     // A/B switch: size pass + full emit pass instead of scratch + gather
+        two_pass = two_pass_env; L = (uint64_t)m->out_chunk_len;
+        if (to_host_stream) B200C_TRY(out_stream_begin(os, c, m->out_compressor, m->out_chunk_len, m->out_max_compressed_len, res->outputs[0].data, res->outputs[0].data_cap, WS_CODEC));
+        return B200C_OK;
+    }
+    int piece(int r) {
         B200C_TRY(check_cancel());
-        // ---- K2 of this piece (Index.db streaming), then its K1 (deferred mode) --------------------------------------------------------
-        if (istream) {
+        if (istream) {                                     // K2 of this piece (Index.db streaming)
             mark(1);
             B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_pool[EV_RANGE + r], 0));
-            B200C_TRY(k2_run(psl[r], psb[r], T[r], T[r + 1]));
+            B200C_TRY(k2(psl[r], psb[r], T[r], T[r + 1]));
         }
         mark(0);
         c->prog_stage.store(1);
-        if (deferred) {
+        if (deferred) {                                    // K1 of this piece
             B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_pool[EV_RANGE + r], 0));
             std::vector<uint64_t> a(K), b(K);
             for (int i = 0; i < K; i++) { a[i] = need[(size_t)r * K + i].k1_a; b[i] = need[(size_t)r * K + i].k1_b; }
             B200C_TRY(k1_many(a, b));
         }
-        // ---- K3: partition merge -------------------------------------------------------------------------------------------------------
+        B200C_TRY(k3(r));
+        B200C_TRY(check_cancel());
+        B200C_TRY(k4());
+        B200C_TRY(check_cancel());
+        B200C_TRY(emit(r));
+        if (want_meta && nparts && ulen_out) B200C_TRY(meta());
+        c->prog_scanned.store(bytes_read * (4 * (uint64_t)r + 3) / (4 * (uint64_t)nr));
+        if (deferred || r == nr - 1) for (int i = 0; i < K; i++) c->prog_input_pos[i].store(range_end[(size_t)r * K + i]);
+        B200C_TRY(k5_stream(r));
+        ubase_total += ulen_out; ilen_total += ilen_out;
+        return B200C_OK;
+    }
+
+    // ---- K3: partition merge; the output partitions counting-sorted by (fan-in, size bucket) ---------------------------------------------
+    int k3(int r) {
         mark(2);
         c->prog_stage.store(3);
         B200C_LAUNCH(c, k_input_ranges, (K + 63) / 64, 64, 0, dP, d_pbase, d_pcount, d_tok, d_upos, T[r], T[r + 1], d_range, (unsigned long long*)nullptr);
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_range, 2 * K * 8, cudaMemcpyDeviceToHost, st));
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 200, d_cerr, 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(P->range, d_range, 2 * K * 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->cerr, d_cerr, 8, cudaMemcpyDeviceToHost, st));
         B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-        if (h[200] != ~0ull) return chunk_error(h[200]);
+        if (P->cerr != ~0ull) return chunk_error(P->cerr);
         uint64_t ncontrib = 0;
-        for (int i = 0; i < K; i++) ncontrib += h[2 * i + 1] - h[2 * i];
+        for (int i = 0; i < K; i++) ncontrib += P->range[2 * i + 1] - P->range[2 * i];
         ncontrib_total += ncontrib;
         const uint64_t nbuckets = std::max<uint64_t>(1, ncontrib / 256);
         uint64_t *d_bstart, *d_opidx; uint32_t* d_head; MergeGeom* d_geom;
@@ -1648,45 +1712,63 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
             B200C_LAUNCH(c, k_bucket_bounds, (unsigned)(((nbuckets + 1) * K + 255) / 256), 256, 0, dP, d_pbase, d_range, d_tok, d_geom, d_bstart);
             B200C_LAUNCH(c, k_merge_buckets, (unsigned)((nbuckets + 3) / 4), 128, 0, dP, d_pbase, d_range, d_tok, d_kp, d_klen, d_upos, d_bstart, nbuckets, d_contrib, d_head, d_hist);
             B200C_TRY(exclusive_scan<uint32_t>(c, d_head, ncontrib, d_opidx, WS_SCANA, 0));
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_opidx + ncontrib, 8, cudaMemcpyDeviceToHost, st));
+            B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->nparts, d_opidx + ncontrib, 8, cudaMemcpyDeviceToHost, st));
             B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-            nparts = h[0];
+            nparts = P->nparts;
         }
         if (nparts >= (1ull << 32)) { c->err = "too many output partitions"; return B200C_EUNSUPPORTED; }
         nparts_total += nparts;
         B200C_TRY(ws_typed(c, WS_OPFIRST, nparts + 2, &d_opfirst));
-        uint32_t* d_list; unsigned long long* d_cursor = nullptr; uint64_t *d_bound = nullptr, *d_bpos = nullptr;
-        uint32_t* d_insz = nullptr; uint8_t* d_big = nullptr;
         B200C_TRY(ws_typed(c, WS_LIST, nparts + 1, &d_list));
         B200C_TRY(ws_typed(c, WS_BOUND, nparts + 1, &d_bound));
         B200C_TRY(ws_typed(c, WS_BPOS, nparts + 2, &d_bpos));
         B200C_TRY(ws_typed(c, WS_ICAP, nparts + 1, &d_icap));
         B200C_TRY(ws_typed(c, WS_IOFF, nparts + 2, &d_ioff));
-        uint64_t n_le8 = 0, n_le12 = 0, n_le16 = 0, n_le32 = 0;
-        if (ncontrib) {
-            B200C_LAUNCH(c, k_op_first, (unsigned)((ncontrib + 1 + 255) / 256), 256, 0, d_head, d_opidx, ncontrib, d_opfirst);
-            // counting sort of the output partitions by (fan-in, size bucket)
-            B200C_TRY(ws_typed(c, WS_INSZ, nparts + 1, &d_insz));
-            B200C_TRY(ws_typed(c, WS_BIG, nparts + 2, &d_big));
-            B200C_LAUNCH(c, k_bounds, (unsigned)((nparts + 255) / 256), 256, 0, d_contrib, d_opfirst, nparts, d_upos, d_pbase, d_bound,
-                         (uint32_t)std::min<uint64_t>(std::max<int64_t>(1, m->column_index_size), 0x7fffffff), d_icap, d_insz, d_big);
-            // tile = token-contiguous run of output partitions whose inputs total ~32 MiB
-            uint64_t per_part = std::max<uint64_t>(1, range_bytes[r] / std::max<uint64_t>(1, nparts));
-            uint32_t tile_shift = 12; while (tile_shift < 24 && ((1ull << (tile_shift + 1)) * per_part) <= (32ull << 20)) tile_shift++;
-            const uint64_t ntiles = (nparts >> tile_shift) + 1, nkeys = 5 * ntiles * SORT_BINS;
-            const uint64_t wide_bound = []() -> uint64_t { const char* e = getenv("B200C_K4_WIDE_WARP"); return e ? strtoull(e, nullptr, 10) : 0; }() ?: ~0ull;    // bytes; unset / 0 = off (A/B)
-            B200C_TRY(ws_typed(c, WS_CURSOR, nkeys + 2, &d_cursor));
-            B200C_CUDA_TRY(c, cudaMemsetAsync(d_cursor, 0, (nkeys + 2) * 8, st));
-            B200C_LAUNCH(c, k_class_hist, 8 * c->nsm, 256, 0, d_opfirst, d_bound, nparts, tile_shift, ntiles, wide_bound, d_cursor);
-            B200C_TRY(exclusive_scan<uint64_t>(c, (const uint64_t*)d_cursor, nkeys, (uint64_t*)d_cursor, WS_SCANA, 0));
-            for (int k = 1; k <= 4; k++) B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 512 + k, (uint64_t*)d_cursor + (uint64_t)k * ntiles * SORT_BINS, 8, cudaMemcpyDeviceToHost, st));
-            B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-            n_le8 = h[513]; n_le12 = h[514]; n_le16 = h[515]; n_le32 = h[516];
-            B200C_LAUNCH(c, k_fanin_scatter, (unsigned)((nparts + 255) / 256), 256, 0, d_opfirst, d_bound, nparts, tile_shift, ntiles, wide_bound, d_cursor, d_list);
-        }
-        B200C_TRY(check_cancel());
+        n_le8 = n_le12 = n_le16 = n_le32 = 0;
+        if (!ncontrib) return B200C_OK;
+        B200C_LAUNCH(c, k_op_first, (unsigned)((ncontrib + 1 + 255) / 256), 256, 0, d_head, d_opidx, ncontrib, d_opfirst);
+        B200C_TRY(ws_typed(c, WS_INSZ, nparts + 1, &d_insz));
+        B200C_TRY(ws_typed(c, WS_BIG, nparts + 2, &d_big));
+        B200C_LAUNCH(c, k_bounds, (unsigned)((nparts + 255) / 256), 256, 0, d_contrib, d_opfirst, nparts, d_upos, d_pbase, d_bound,
+                     (uint32_t)std::min<uint64_t>(std::max<int64_t>(1, m->column_index_size), 0x7fffffff), d_icap, d_insz, d_big);
+        // tile = token-contiguous run of output partitions whose inputs total ~32 MiB
+        uint64_t per_part = std::max<uint64_t>(1, range_bytes[r] / std::max<uint64_t>(1, nparts));
+        uint32_t tile_shift = 12; while (tile_shift < 24 && ((1ull << (tile_shift + 1)) * per_part) <= (32ull << 20)) tile_shift++;
+        const uint64_t ntiles = (nparts >> tile_shift) + 1, nkeys = 5 * ntiles * SORT_BINS;
+        const uint64_t wide_bound = []() -> uint64_t { const char* e = getenv("B200C_K4_WIDE_WARP"); return e ? strtoull(e, nullptr, 10) : 0; }() ?: ~0ull;    // bytes; unset / 0 = off (A/B)
+        unsigned long long* d_cursor;
+        B200C_TRY(ws_typed(c, WS_CURSOR, nkeys + 2, &d_cursor));
+        B200C_CUDA_TRY(c, cudaMemsetAsync(d_cursor, 0, (nkeys + 2) * 8, st));
+        B200C_LAUNCH(c, k_class_hist, 8 * c->nsm, 256, 0, d_opfirst, d_bound, nparts, tile_shift, ntiles, wide_bound, d_cursor);
+        B200C_TRY(exclusive_scan<uint64_t>(c, (const uint64_t*)d_cursor, nkeys, (uint64_t*)d_cursor, WS_SCANA, 0));
+        for (int k = 1; k <= 4; k++) B200C_CUDA_TRY(c, cudaMemcpyAsync(P->class_end + k - 1, (uint64_t*)d_cursor + (uint64_t)k * ntiles * SORT_BINS, 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
+        n_le8 = P->class_end[0]; n_le12 = P->class_end[1]; n_le16 = P->class_end[2]; n_le32 = P->class_end[3];
+        B200C_LAUNCH(c, k_fanin_scatter, (unsigned)((nparts + 255) / 256), 256, 0, d_opfirst, d_bound, nparts, tile_shift, ntiles, wide_bound, d_cursor, d_list);
+        return B200C_OK;
+    }
 
-        // ---- K4: row merge + serialise ---------------------------------------------------------------------------------------------------
+    // ---- K4: row merge + serialise ---------------------------------------------------------------------------------------------------
+    // one launch per fan-in class over its slice of the sorted list
+    int launch_k4(int mode) {
+        ka.mode = mode;
+        const bool emit = mode != 0;
+        if (hp.ncx || hp.ctr_mask || hp.sctr_mask) {
+            // tables with multi-cell (complex) or counter columns: the CX instantiations of the thread kernels, for every fan-in (64 cursors per thread above 16);
+            // single serialisation pass only (the size-pass A/B mode is refused above)
+            if (!emit) { c->err = "B200C_K4_TWO_PASS with multi-cell columns"; return B200C_EUNSUPPORTED; }
+            B200C_TRY((k4_thr<8, 128, true>(c, ka, true, 0, n_le8, smem8)));
+            B200C_TRY((k4_thr<12, 64, true>(c, ka, true, n_le8, n_le12, smem12)));
+            B200C_TRY((k4_thr<16, 64, true>(c, ka, true, n_le12, n_le16, smem16)));
+            return k4_thr<64, 32, true>(c, ka, true, n_le16, nparts, smem64);
+        }
+        B200C_TRY((k4_thr<8, 128>(c, ka, emit, 0, n_le8, smem8)));
+        B200C_TRY((k4_thr<12, 64>(c, ka, emit, n_le8, n_le12, smem12)));
+        B200C_TRY((k4_thr<16, 64>(c, ka, emit, n_le12, n_le16, smem16)));
+        B200C_TRY(k4_warp<1>(c, ka, emit, n_le16, n_le32, cell_smem32));
+        return k4_warp<2>(c, ka, emit, n_le32, nparts, cell_smem32);
+    }
+    int k4() {
         mark(3);
         c->prog_stage.store(4);
         B200C_TRY(ws_typed(c, WS_DSIZE, nparts + 1, &d_dsize));
@@ -1700,261 +1782,202 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         B200C_TRY(ws_typed(c, WS_STROWS, nparts + 1, &d_strows));
         B200C_TRY(ws_typed(c, WS_OVF, nparts + 1, &d_ovf));
         const size_t cols_s = hp.mcols <= K4_SMEM_COLS ? (size_t)hp.mcols * sizeof(MCell) : 0;
-        const size_t smem8 = (size_t)128 * (8 * SLOT_BYTES + cols_s + 8), smem12 = (size_t)64 * (12 * SLOT_BYTES + cols_s + 8), smem16 = (size_t)64 * (16 * SLOT_BYTES + cols_s + 8), smem64 = (size_t)32 * (64 * SLOT_BYTES + cols_s + 8), cell_smem32 = (size_t)4 * hp.mcols * sizeof(MCell);
+        smem8 = (size_t)128 * (8 * SLOT_BYTES + cols_s + 8); smem12 = (size_t)64 * (12 * SLOT_BYTES + cols_s + 8); smem16 = (size_t)64 * (16 * SLOT_BYTES + cols_s + 8);
+        smem64 = (size_t)32 * (64 * SLOT_BYTES + cols_s + 8); cell_smem32 = (size_t)4 * hp.mcols * sizeof(MCell);
         memset(&ka, 0, sizeof(ka));
         ka.P = dP; ka.contrib = d_contrib; ka.op_first = d_opfirst; ka.list = d_list; ka.upos = d_upos; ka.pbase = d_pbase; ka.kp = d_kp; ka.klen = d_klen; ka.tok = d_tok;
         ka.dsize = d_dsize; ka.ipay = d_ipay; ka.nblk = d_nblk; ka.ihead = d_ihead; ka.st_munf = d_stmunf; ka.st_rows = d_strows; ka.ovf = d_ovf;
         ka.dpos = d_dpos; ka.ipos = d_ipos; ka.err = d_err; ka.jlo = 0; ka.jhi = nparts; ka.m3_nblk = two_pass ? 1 : 0;
-        uint32_t* d_ccount = nullptr; uint32_t* d_wflag = nullptr; uint64_t* d_wrank = nullptr;
         if (want_meta) {
             B200C_TRY(ws_typed(c, WS_CCOUNT, nparts + 1, &d_ccount));
             B200C_TRY(ws_typed(c, WS_META_FLAG, nparts + 1, &d_wflag));
             B200C_TRY(ws_typed(c, WS_META_WRANK, nparts + 2, &d_wrank));
             ka.sg = d_sg; ka.td = d_td; ka.ccount = d_ccount;
         }
-        // one launch per fan-in class over its slice of the sorted list
-        const uint64_t np_ = nparts;
-        launch_k4 = [&, n_le8, n_le12, n_le16, n_le32, np_, smem8, smem12, smem16, smem64, cell_smem32](int mode) -> int {
-            ka.mode = mode;
-            const bool emit = mode != 0;
-            if (hp.ncx || hp.ctr_mask || hp.sctr_mask) {
-                // tables with multi-cell (complex) or counter columns: the CX instantiations of the thread kernels, for every fan-in (64 cursors per thread above 16);
-                // single serialisation pass only (the size-pass A/B mode is refused above)
-                if (!emit) { c->err = "B200C_K4_TWO_PASS with multi-cell columns"; return B200C_EUNSUPPORTED; }
-                if (n_le8) B200C_LAUNCH(c, (k_partition_thr<8, 128, true, true>), (unsigned)((n_le8 + 127) / 128), 128, smem8, ka, 0ull, n_le8);
-                if (n_le12 > n_le8) B200C_LAUNCH(c, (k_partition_thr<12, 64, true, true>), (unsigned)((n_le12 - n_le8 + 63) / 64), 64, smem12, ka, n_le8, n_le12);
-                if (n_le16 > n_le12) B200C_LAUNCH(c, (k_partition_thr<16, 64, true, true>), (unsigned)((n_le16 - n_le12 + 63) / 64), 64, smem16, ka, n_le12, n_le16);
-                if (np_ > n_le16) B200C_LAUNCH(c, (k_partition_thr<64, 32, true, true>), (unsigned)((np_ - n_le16 + 31) / 32), 32, smem64, ka, n_le16, np_);
-                return B200C_OK;
-            }
-            if (n_le8) {
-                unsigned g = (unsigned)((n_le8 + 127) / 128);
-                if (emit) B200C_LAUNCH(c, (k_partition_thr<8, 128, true>), g, 128, smem8, ka, 0ull, n_le8);
-                else B200C_LAUNCH(c, (k_partition_thr<8, 128, false>), g, 128, smem8, ka, 0ull, n_le8);
-            }
-            if (n_le12 > n_le8) {
-                unsigned g = (unsigned)((n_le12 - n_le8 + 63) / 64);
-                if (emit) B200C_LAUNCH(c, (k_partition_thr<12, 64, true>), g, 64, smem12, ka, n_le8, n_le12);
-                else B200C_LAUNCH(c, (k_partition_thr<12, 64, false>), g, 64, smem12, ka, n_le8, n_le12);
-            }
-            if (n_le16 > n_le12) {
-                unsigned g = (unsigned)((n_le16 - n_le12 + 63) / 64);
-                if (emit) B200C_LAUNCH(c, (k_partition_thr<16, 64, true>), g, 64, smem16, ka, n_le12, n_le16);
-                else B200C_LAUNCH(c, (k_partition_thr<16, 64, false>), g, 64, smem16, ka, n_le12, n_le16);
-            }
-            if (n_le32 > n_le16) {
-                unsigned g = (unsigned)((n_le32 - n_le16 + 3) / 4);
-                if (emit) B200C_LAUNCH(c, (k_partition_warp<1, true>), g, 128, cell_smem32, ka, n_le16, n_le32);
-                else B200C_LAUNCH(c, (k_partition_warp<1, false>), g, 128, cell_smem32, ka, n_le16, n_le32);
-            }
-            if (np_ > n_le32) {
-                unsigned g = (unsigned)((np_ - n_le32 + 3) / 4);
-                if (emit) B200C_LAUNCH(c, (k_partition_warp<2, true>), g, 128, cell_smem32, ka, n_le32, np_);
-                else B200C_LAUNCH(c, (k_partition_warp<2, false>), g, 128, cell_smem32, ka, n_le32, np_);
-            }
-            return B200C_OK;
-        };
-        if (c->k4_attr_set != (int)(smem8 + 1)) {      // > 48 KiB of dynamic shared memory needs an explicit opt-in, once per context/device
-            cudaFuncSetAttribute(k_partition_thr<8, 128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem8);
-            cudaFuncSetAttribute(k_partition_thr<8, 128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem8);
-            cudaFuncSetAttribute(k_partition_thr<12, 64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem12);
-            cudaFuncSetAttribute(k_partition_thr<12, 64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem12);
-            cudaFuncSetAttribute(k_partition_thr<16, 64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16);
-            cudaFuncSetAttribute(k_partition_thr<16, 64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16);
-            cudaFuncSetAttribute(k_partition_thr<8, 128, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem8);
-            cudaFuncSetAttribute(k_partition_thr<12, 64, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem12);
-            cudaFuncSetAttribute(k_partition_thr<16, 64, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16);
-            cudaFuncSetAttribute(k_partition_thr<64, 32, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem64);
-            // B200C_K4_CARVEOUT=percent of the SM's unified L1/shared memory left to shared memory (A/B: fewer resident blocks, more L1 for the
-            // scattered reads of Data.db); unset: the driver sizes the carve-out for the most blocks that fit
-            if (const char* e = getenv("B200C_K4_CARVEOUT")) { const int pct = atoi(e);
-                cudaFuncSetAttribute(k_partition_thr<8, 128, true>, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-                cudaFuncSetAttribute(k_partition_thr<12, 64, true>, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-                cudaFuncSetAttribute(k_partition_thr<16, 64, true>, cudaFuncAttributePreferredSharedMemoryCarveout, pct); }
+        if (c->k4_attr_set != (int)(smem8 + 1)) {          // once per context / device and shared memory size
+            const char* carveout = getenv("B200C_K4_CARVEOUT");
+            k4_attr<8, 128, true>(smem8, carveout); k4_attr<8, 128, false>(smem8); k4_attr<8, 128, true, true>(smem8);
+            k4_attr<12, 64, true>(smem12, carveout); k4_attr<12, 64, false>(smem12); k4_attr<12, 64, true, true>(smem12);
+            k4_attr<16, 64, true>(smem16, carveout); k4_attr<16, 64, false>(smem16); k4_attr<16, 64, true, true>(smem16);
+            k4_attr<64, 32, true, true>(smem64);
             c->k4_attr_set = (int)(smem8 + 1);
         }
-        uint8_t* SCRATCH = nullptr;
         ulen_out = 0; ilen_out = 0;
-        if (nparts) {
-            if (two_pass) {
-                B200C_CUDA_TRY(c, cudaMemsetAsync(d_ovf, 0, nparts, st));
-                B200C_TRY(launch_k4(0));
-            } else {
-                B200C_TRY(exclusive_scan<uint64_t>(c, d_bound, nparts, d_bpos, WS_SCANA, 0));
-                B200C_TRY(exclusive_scan<uint32_t>(c, d_icap, nparts, d_ioff, WS_SCANA + 3, 0));
-                B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_bpos + nparts, 8, cudaMemcpyDeviceToHost, st));
-                B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 1, d_ioff + nparts, 8, cudaMemcpyDeviceToHost, st));
-                B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-                B200C_TRY(ws_typed(c, WS_SCRATCH, h[0] + 64, &SCRATCH));
-                B200C_TRY(ws_typed(c, WS_ISCR, h[1] + 64, &ISCR));
-                ka.doff = d_bpos; ka.dcapv = d_bound; ka.dbase = SCRATCH; ka.iout = nullptr; ka.ioff = d_ioff; ka.icapv = d_icap; ka.iscr = ISCR;
-                const bool staged = !hp.ncx && !hp.ctr_mask && !hp.sctr_mask && []() { const char* e = getenv("B200C_K4_STAGED"); return e ? atoi(e) != 0 : (B200C_K4_STAGED_DEFAULT != 0); }();      // A/B switch (read per call; tables with multi-cell columns: thread kernels)
-                if (staged) {
-                    // tile plan: exclusive scan of the input bytes, cut marks, scan of the marks, tile starts
-                    uint64_t *d_inpos, *d_tscan; uint32_t *d_mark, *d_tstart; unsigned long long* d_nbig = (unsigned long long*)(d_stats + 1);
-                    B200C_TRY(ws_typed(c, WS_INPOS, nparts + 2, &d_inpos));
-                    B200C_TRY(ws_typed(c, WS_TMARK, nparts + 2, &d_mark));
-                    B200C_TRY(ws_typed(c, WS_TSCAN, nparts + 2, &d_tscan));
-                    B200C_TRY(ws_typed(c, WS_TSTART, nparts + 2, &d_tstart));
-                    B200C_TRY(exclusive_scan<uint32_t>(c, d_insz, nparts, d_inpos, WS_SCANA, 0));
-                    B200C_CUDA_TRY(c, cudaMemsetAsync(d_nbig, 0, 8, st));
-                    B200C_LAUNCH(c, k_tile_marks, (unsigned)((nparts + 255) / 256), 256, 0, nparts, d_inpos, d_opfirst, d_big, d_mark, d_nbig);
-                    B200C_TRY(exclusive_scan<uint32_t>(c, d_mark, nparts, d_tscan, WS_SCANA, 0));
-                    B200C_LAUNCH(c, k_tile_starts, (unsigned)((nparts + 1 + 255) / 256), 256, 0, nparts, d_mark, d_tscan, d_tstart);
-                    B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_tscan + nparts, 8, cudaMemcpyDeviceToHost, st));
-                    B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 1, d_nbig, 8, cudaMemcpyDeviceToHost, st));
-                    B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-                    const uint64_t ntiles = h[0], nbig = h[1];
-                    const bool wide = m->ncolumns > K4_SMEM_COLS;
-                    const size_t smem_st = (size_t)ST_HEAD + ST_STAGE_CAP + (size_t)ST_CUR_CAP * sizeof(CurS) + (wide ? 0 : (size_t)ST_THREADS * hp.mcols * sizeof(MCell)) + 16;
-                    if (c->k4s_attr_set != (int)smem_st) {
-                        cudaFuncSetAttribute(k_partition_staged<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_st);
-                        cudaFuncSetAttribute(k_partition_staged<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_st);
-                        c->k4s_attr_set = (int)smem_st;
-                    }
-                    ka.mode = 1; ka.only_big = nullptr;
-                    if (wide) B200C_LAUNCH(c, k_partition_staged<true>, (unsigned)ntiles, ST_THREADS, smem_st, ka, d_tstart, d_big);
-                    else B200C_LAUNCH(c, k_partition_staged<false>, (unsigned)ntiles, ST_THREADS, smem_st, ka, d_tstart, d_big);
-                    if (nbig) { ka.only_big = d_big; B200C_TRY(launch_k4(1)); ka.only_big = nullptr; }
-                } else B200C_TRY(launch_k4(1));
-            }
-            B200C_LAUNCH(c, k_sum_stats, 8 * c->nsm, 256, 0, nparts, d_dsize, d_stmunf, d_strows, d_stats);
-            B200C_TRY(exclusive_scan<uint64_t>(c, d_dsize, nparts, d_dpos, WS_SCANA, 0));
-            if (ubase_total) B200C_LAUNCH(c, k_add_u64, (unsigned)((nparts + 1 + 255) / 256), 256, 0, d_dpos, nparts + 1, ubase_total);     // positions in the file, not in the piece
-            B200C_LAUNCH(c, k_index_sizes, (unsigned)((nparts + 255) / 256), 256, 0, nparts, d_dsize, d_dpos, d_ipay, d_ihead, d_isize);
-            B200C_TRY(exclusive_scan<uint32_t>(c, d_isize, nparts, d_ipos, WS_SCANA + 3, 0));
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_dpos + nparts, 8, cudaMemcpyDeviceToHost, st));
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 1, d_ipos + nparts, 8, cudaMemcpyDeviceToHost, st));
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 2, d_err, 8, cudaMemcpyDeviceToHost, st));
-            if (want_meta) {
-                B200C_LAUNCH(c, k_written_flags, (unsigned)((nparts + 255) / 256), 256, 0, nparts, d_dsize, d_wflag);
-                B200C_TRY(exclusive_scan<uint32_t>(c, d_wflag, nparts, d_wrank, WS_SCANA, 0));
-                B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 3, d_wrank + nparts, 8, cudaMemcpyDeviceToHost, st));
-            }
-            B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-            if (h[2] != ~0ull) {
-                int kinde = (int)(h[2] >> 56);
-                res->corruption.input = (int)((h[2] >> 48) & 0xFF); res->corruption.kind = 4; res->corruption.chunk = 0; res->corruption.offset = h[2] & 0xFFFFFFFFFFFFull;
-                timing_end(c);
-                if (kinde == 9) { c->err = "unsupported feature in input " + std::to_string(res->corruption.input) + " (outside the envelope: shadowable deletion, a fan-in or layout the kernels refuse, or a counter context the reference never writes inside a merge)"; return B200C_EUNSUPPORTED; }
-                c->err = "malformed Data.db in input " + std::to_string(res->corruption.input) + " near offset " + std::to_string(res->corruption.offset);
-                return B200C_ECORRUPT;
-            }
-            ulen_out = h[0] - ubase_total; ilen_out = h[1];
+        if (!nparts) return B200C_OK;
+        if (two_pass) {
+            B200C_CUDA_TRY(c, cudaMemsetAsync(d_ovf, 0, nparts, st));
+            B200C_TRY(launch_k4(0));
+        } else B200C_TRY(k4_scratch());
+        B200C_LAUNCH(c, k_sum_stats, 8 * c->nsm, 256, 0, nparts, d_dsize, d_stmunf, d_strows, d_stats);
+        B200C_TRY(exclusive_scan<uint64_t>(c, d_dsize, nparts, d_dpos, WS_SCANA, 0));
+        if (ubase_total) B200C_LAUNCH(c, k_add_u64, (unsigned)((nparts + 1 + 255) / 256), 256, 0, d_dpos, nparts + 1, ubase_total);     // positions in the file, not in the piece
+        B200C_LAUNCH(c, k_index_sizes, (unsigned)((nparts + 255) / 256), 256, 0, nparts, d_dsize, d_dpos, d_ipay, d_ihead, d_isize);
+        B200C_TRY(exclusive_scan<uint32_t>(c, d_isize, nparts, d_ipos, WS_SCANA + 3, 0));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->data_end, d_dpos + nparts, 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->index_len, d_ipos + nparts, 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->err, d_err, 8, cudaMemcpyDeviceToHost, st));
+        if (want_meta) {
+            B200C_LAUNCH(c, k_written_flags, (unsigned)((nparts + 255) / 256), 256, 0, nparts, d_dsize, d_wflag);
+            B200C_TRY(exclusive_scan<uint32_t>(c, d_wflag, nparts, d_wrank, WS_SCANA, 0));
+            B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->written, d_wrank + nparts, 8, cudaMemcpyDeviceToHost, st));
         }
-        B200C_TRY(check_cancel());
+        B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
+        if (P->err != ~0ull) {
+            const int in = (int)((P->err >> 48) & 0xFF); const uint64_t off = P->err & 0xFFFFFFFFFFFFull;
+            if ((int)(P->err >> 56) == 9) { corrupt(in, 4, 0, off, ""); c->err = "unsupported feature in input " + std::to_string(in) + " (outside the envelope: shadowable deletion, a fan-in or layout the kernels refuse, or a counter context the reference never writes inside a merge)"; return B200C_EUNSUPPORTED; }
+            return corrupt(in, 4, 0, off, "malformed Data.db in input " + std::to_string(in) + " near offset " + std::to_string(off));
+        }
+        ulen_out = P->data_end - ubase_total; ilen_out = P->index_len;
+        return B200C_OK;
+    }
+    // every partition serialised into its scratch slot (bounded by its inputs); k_gather moves them into place once positions are known
+    int k4_scratch() {
+        B200C_TRY(exclusive_scan<uint64_t>(c, d_bound, nparts, d_bpos, WS_SCANA, 0));
+        B200C_TRY(exclusive_scan<uint32_t>(c, d_icap, nparts, d_ioff, WS_SCANA + 3, 0));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->scratch_len, d_bpos + nparts, 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->iscr_len, d_ioff + nparts, 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
+        B200C_TRY(ws_typed(c, WS_SCRATCH, P->scratch_len + 64, &SCRATCH));
+        B200C_TRY(ws_typed(c, WS_ISCR, P->iscr_len + 64, &ISCR));
+        ka.doff = d_bpos; ka.dcapv = d_bound; ka.dbase = SCRATCH; ka.iout = nullptr; ka.ioff = d_ioff; ka.icapv = d_icap; ka.iscr = ISCR;
+        const bool staged = !hp.ncx && !hp.ctr_mask && !hp.sctr_mask && []() { const char* e = getenv("B200C_K4_STAGED"); return e ? atoi(e) != 0 : (B200C_K4_STAGED_DEFAULT != 0); }();      // A/B switch (read per call; tables with multi-cell columns: thread kernels)
+        if (!staged) return launch_k4(1);
+        // tile plan: exclusive scan of the input bytes, cut marks, scan of the marks, tile starts
+        uint64_t *d_inpos, *d_tscan; uint32_t *d_mark, *d_tstart; unsigned long long* d_nbig = (unsigned long long*)(d_stats + 1);
+        B200C_TRY(ws_typed(c, WS_INPOS, nparts + 2, &d_inpos));
+        B200C_TRY(ws_typed(c, WS_TMARK, nparts + 2, &d_mark));
+        B200C_TRY(ws_typed(c, WS_TSCAN, nparts + 2, &d_tscan));
+        B200C_TRY(ws_typed(c, WS_TSTART, nparts + 2, &d_tstart));
+        B200C_TRY(exclusive_scan<uint32_t>(c, d_insz, nparts, d_inpos, WS_SCANA, 0));
+        B200C_CUDA_TRY(c, cudaMemsetAsync(d_nbig, 0, 8, st));
+        B200C_LAUNCH(c, k_tile_marks, (unsigned)((nparts + 255) / 256), 256, 0, nparts, d_inpos, d_opfirst, d_big, d_mark, d_nbig);
+        B200C_TRY(exclusive_scan<uint32_t>(c, d_mark, nparts, d_tscan, WS_SCANA, 0));
+        B200C_LAUNCH(c, k_tile_starts, (unsigned)((nparts + 1 + 255) / 256), 256, 0, nparts, d_mark, d_tscan, d_tstart);
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->ntiles, d_tscan + nparts, 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->nbig, d_nbig, 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
+        const bool wide = m->ncolumns > K4_SMEM_COLS;
+        const size_t smem_st = (size_t)ST_HEAD + ST_STAGE_CAP + (size_t)ST_CUR_CAP * sizeof(CurS) + (wide ? 0 : (size_t)ST_THREADS * hp.mcols * sizeof(MCell)) + 16;
+        if (c->k4s_attr_set != (int)smem_st) { k4_staged_attr<false>(smem_st); k4_staged_attr<true>(smem_st); c->k4s_attr_set = (int)smem_st; }
+        ka.mode = 1; ka.only_big = nullptr;
+        B200C_TRY(wide ? k4_staged<true>(c, ka, P->ntiles, smem_st, d_tstart, d_big) : k4_staged<false>(c, ka, P->ntiles, smem_st, d_tstart, d_big));
+        if (P->nbig) { ka.only_big = d_big; B200C_TRY(launch_k4(1)); ka.only_big = nullptr; }
+        return B200C_OK;
+    }
+    // the piece's Data.db and Index.db in place: the merged stream goes behind the unconsumed tail of the previous piece; UOUT + tail_len is
+    // file offset ubase_total
+    int emit(int r) {
         mark(4);
-        // the merged stream of this piece goes behind the unconsumed tail of the previous one; UOUT + tail_len is file offset ubase_total
-        if (k5_async && r >= 2) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_pool[EV_K5 + 1 + (r & 1)], 0));      // K5 of piece r - 2 has read this buffer
-        if (raw_out && to_host_stream && r >= 2) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_pool[EV_K5 + 1 + (r & 1)], 0));      // piece r - 2's bytes have left it
+        if (raw_out && to_host_stream && r >= 2) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_pool[EV_UOUT_FREE + (r & 1)], 0));      // piece r - 2's bytes have left it
         B200C_TRY(ws_typed(c, (r & 1) ? WS_UOUT2 : WS_UOUT, tail_len + ulen_out + 64, &UOUT));
-        if (r) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_pool[EV_INDEX], 0));          // IOUT of the previous piece has left
+        if (r) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_pool[EV_INDEX_FREE], 0));          // IOUT of the previous piece has left
         B200C_TRY(ws_typed(c, WS_IOUT, ilen_out + 64, &IOUT));
         if (tail_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(UOUT, tail_ptr, tail_len, cudaMemcpyDeviceToDevice, st));
         uint8_t* const ubias = (uint8_t*)((uintptr_t)UOUT + tail_len - ubase_total);          // ubias + (file offset) = address
-        if (nparts && ulen_out) {
-            ka.dbase = ubias; ka.iout = IOUT; ka.doff = nullptr; ka.dcapv = nullptr;
-            if (two_pass) B200C_TRY(launch_k4(2));
-            else {
-                B200C_LAUNCH(c, k_gather, (unsigned)((nparts + 7) / 8), 256, 0, nparts, d_dsize, d_dpos, d_bpos, d_ovf, SCRATCH, ubias);
-                B200C_LAUNCH(c, k_index_simple, (unsigned)((nparts + 255) / 256), 256, 0, dP, nparts, d_contrib, d_opfirst, d_upos, d_pbase, d_dsize, d_dpos, d_nblk, d_ovf, d_ihead, d_ipos, IOUT);
-                B200C_LAUNCH(c, k_index_promoted, (unsigned)((nparts + 127) / 128), 128, 0, dP, nparts, d_contrib, d_opfirst, d_upos, d_pbase, d_dsize, d_dpos, d_nblk, d_ovf, d_ihead, d_ipay, d_ipos,
-                             d_ioff, d_icap, ISCR, IOUT);
-                B200C_TRY(launch_k4(3));
-            }
+        if (!nparts || !ulen_out) return B200C_OK;
+        ka.dbase = ubias; ka.iout = IOUT; ka.doff = nullptr; ka.dcapv = nullptr;
+        if (two_pass) return launch_k4(2);
+        B200C_LAUNCH(c, k_gather, (unsigned)((nparts + 7) / 8), 256, 0, nparts, d_dsize, d_dpos, d_bpos, d_ovf, SCRATCH, ubias);
+        B200C_LAUNCH(c, k_index_simple, (unsigned)((nparts + 255) / 256), 256, 0, dP, nparts, d_contrib, d_opfirst, d_upos, d_pbase, d_dsize, d_dpos, d_nblk, d_ovf, d_ihead, d_ipos, IOUT);
+        B200C_LAUNCH(c, k_index_promoted, (unsigned)((nparts + 127) / 128), 128, 0, dP, nparts, d_contrib, d_opfirst, d_upos, d_pbase, d_dsize, d_dpos, d_nblk, d_ovf, d_ihead, d_ipay, d_ipos,
+                     d_ioff, d_icap, ISCR, IOUT);
+        return launch_k4(3);
+    }
+    // per key / per partition metadata of this piece: bloom bits, HLL registers, histograms, index-summary samples, first / last key
+    int meta() {
+        const uint64_t ns = (written_total + P->written + meta_interval - 1) / meta_interval - (written_total + meta_interval - 1) / meta_interval;
+        uint32_t *d_samplej, *d_esize; uint64_t* d_epos;
+        B200C_TRY(ws_typed(c, WS_META_SAMPLE, ns + 1, &d_samplej));
+        B200C_TRY(ws_typed(c, WS_META_ESIZE, ns + 1, &d_esize));
+        B200C_TRY(ws_typed(c, WS_META_EPOS, ns + 2, &d_epos));
+        MetaArgs ma; memset(&ma, 0, sizeof(ma));
+        ma.P = dP; ma.contrib = d_contrib; ma.op_first = d_opfirst; ma.upos = d_upos; ma.pbase = d_pbase; ma.dsize = d_dsize; ma.ipos = d_ipos; ma.ihead = d_ihead;
+        ma.ccount = d_ccount; ma.wrank = d_wrank; ma.nparts = nparts; ma.index_base = ilen_total; ma.written_base = written_total; ma.sg = d_sg;
+        ma.bloom = d_bloom; ma.bloom_bits = bloom_words * 64; ma.bloom_k = m->bloom_hash_count; ma.interval = meta_interval; ma.sample_j = d_samplej;
+        ma.first_key = d_mkeys; ma.last_key = d_mkeys + 65536;
+        B200C_LAUNCH(c, k_meta_keys, (unsigned)((nparts + 255) / 256), 256, 0, ma);
+        if (ns && res->outputs[0].summary) {
+            B200C_LAUNCH(c, k_summary_sizes, (unsigned)((ns + 255) / 256), 256, 0, ma, ns, d_esize);
+            B200C_TRY(exclusive_scan<uint32_t>(c, d_esize, ns, d_epos, WS_SCANA, 0));
+            B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->summary_len, d_epos + ns, 8, cudaMemcpyDeviceToHost, st));
+            B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
+            B200C_TRY(ws_grow_keep<uint8_t>(c, WS_META_SUMENT, sument_bound + P->summary_len + 64, sument_bound, &d_sument));
+            B200C_TRY(ws_grow_keep<uint64_t>(c, WS_META_SUMOFF, samples_total + ns + 2, samples_total, &d_sumoff));
+            B200C_LAUNCH(c, k_summary_emit, (unsigned)((ns + 255) / 256), 256, 0, ma, ns, d_epos, d_sument, d_sumoff);
+            B200C_LAUNCH(c, k_meta_advance, 1, 1, 0, d_sg, ns, d_epos);
+            sument_bound += P->summary_len; samples_total += ns;
         }
-        if (want_meta && nparts && ulen_out) {
-            // per key / per partition metadata of this piece: bloom bits, HLL registers, histograms, index-summary samples, first / last key
-            const uint64_t nwritten = h[3];
-            const uint64_t ns = (written_total + nwritten + meta_interval - 1) / meta_interval - (written_total + meta_interval - 1) / meta_interval;
-            uint32_t *d_samplej, *d_esize; uint64_t* d_epos;
-            B200C_TRY(ws_typed(c, WS_META_SAMPLE, ns + 1, &d_samplej));
-            B200C_TRY(ws_typed(c, WS_META_ESIZE, ns + 1, &d_esize));
-            B200C_TRY(ws_typed(c, WS_META_EPOS, ns + 2, &d_epos));
-            MetaArgs ma; memset(&ma, 0, sizeof(ma));
-            ma.P = dP; ma.contrib = d_contrib; ma.op_first = d_opfirst; ma.upos = d_upos; ma.pbase = d_pbase; ma.dsize = d_dsize; ma.ipos = d_ipos; ma.ihead = d_ihead;
-            ma.ccount = d_ccount; ma.wrank = d_wrank; ma.nparts = nparts; ma.index_base = ilen_total; ma.written_base = written_total; ma.sg = d_sg;
-            ma.bloom = d_bloom; ma.bloom_bits = bloom_words * 64; ma.bloom_k = m->bloom_hash_count; ma.interval = meta_interval; ma.sample_j = d_samplej;
-            ma.first_key = d_mkeys; ma.last_key = d_mkeys + 65536;
-            B200C_LAUNCH(c, k_meta_keys, (unsigned)((nparts + 255) / 256), 256, 0, ma);
-            if (ns && o0.summary) {
-                B200C_LAUNCH(c, k_summary_sizes, (unsigned)((ns + 255) / 256), 256, 0, ma, ns, d_esize);
-                B200C_TRY(exclusive_scan<uint32_t>(c, d_esize, ns, d_epos, WS_SCANA, 0));
-                B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 4, d_epos + ns, 8, cudaMemcpyDeviceToHost, st));
-                B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-                B200C_TRY(ws_grow_keep<uint8_t>(c, WS_META_SUMENT, sument_bound + h[4] + 64, sument_bound, &d_sument));
-                B200C_TRY(ws_grow_keep<uint64_t>(c, WS_META_SUMOFF, samples_total + ns + 2, samples_total, &d_sumoff));
-                B200C_LAUNCH(c, k_summary_emit, (unsigned)((ns + 255) / 256), 256, 0, ma, ns, d_epos, d_sument, d_sumoff);
-                B200C_LAUNCH(c, k_meta_advance, 1, 1, 0, d_sg, ns, d_epos);
-                sument_bound += h[4]; samples_total += ns;
-            }
-            written_total += nwritten;
-        }
-        c->prog_scanned.store(bytes_read * (4 * (uint64_t)r + 3) / (4 * (uint64_t)nr));
-        if (deferred || r == nr - 1) for (int i = 0; i < K; i++) c->prog_input_pos[i].store(range_end[(size_t)r * K + i]);
-
-        // ---- K5 of this piece (one output file in host memory): whole chunks go out now, the rest waits for the next piece -------------
+        written_total += P->written;
+        return B200C_OK;
+    }
+    // ---- K5 of this piece (one output file in host memory): whole chunks go out now, the rest waits for the next piece -----------------
+    int k5_stream(int r) {
         mark(5);
         c->prog_stage.store(5);
-        if (to_host_stream) {
-            if (ilen_out) {                                  // Index.db is final after K4: read it back while K5 compresses
-                if (ilen_total + ilen_out > out0.index_cap || !out0.index) index_fits = false;
-                if (index_fits) {
-                    B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_INDEX + 1], st));
-                    B200C_CUDA_TRY(c, cudaStreamWaitEvent(c->copy_out, c->ev_pool[EV_INDEX + 1], 0));
-                    B200C_CUDA_TRY(c, cudaMemcpyAsync(out0.index + ilen_total, IOUT, ilen_out, cudaMemcpyDeviceToHost, c->copy_out));
-                }
+        if (!to_host_stream) return B200C_OK;
+        b200c_output& out0 = res->outputs[0];
+        if (ilen_out) {                                  // Index.db is final after K4: read it back while K5 compresses
+            if (ilen_total + ilen_out > out0.index_cap || !out0.index) index_fits = false;
+            if (index_fits) {
+                B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_INDEX_READY], st));
+                B200C_CUDA_TRY(c, cudaStreamWaitEvent(c->copy_out, c->ev_pool[EV_INDEX_READY], 0));
+                B200C_CUDA_TRY(c, cudaMemcpyAsync(out0.index + ilen_total, IOUT, ilen_out, cudaMemcpyDeviceToHost, c->copy_out));
             }
-            B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_INDEX], c->copy_out));
-            const uint64_t avail = tail_len + ulen_out;
-            uint64_t take = (r == nr - 1) ? avail : avail / L * L;
-            const uint64_t slice = std::max<uint64_t>(L, std::max<uint64_t>(512ull << 20, bytes_read / 32) / L * L);      // pieces of ~512 MiB keep the read-back close behind
-            if (k5_async) {
-                // K5 of this piece on its own stream: it needs UOUT only, so K1..K3 of the next piece — and the host->device copies they wait for —
-                // run on top of it; K4 of piece r + 2 waits for it before it reuses this UOUT buffer
-                B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_K5], st));
-                B200C_CUDA_TRY(c, cudaStreamWaitEvent(c->stream5, c->ev_pool[EV_K5], 0));
-                while (c->ev_k5.size() < k5_marks + 2) { cudaEvent_t e; cudaEventCreate(&e); c->ev_k5.push_back(e); }
-                cudaEventRecord(c->ev_k5[k5_marks], c->stream5);
-                c->stream = c->stream5;
-            }
-            int arc = B200C_OK;
-            for (uint64_t off = 0; off < take && arc == B200C_OK; off += slice) arc = out_stream_append(os, UOUT + off, std::min(slice, take - off));
-            if (k5_async) {
-                c->stream = st;
-                cudaEventRecord(c->ev_k5[k5_marks + 1], c->stream5); k5_marks += 2;
-                B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_K5 + 1 + (r & 1)], c->stream5));
-                k5_last = EV_K5 + 1 + (r & 1);
-            }
-            B200C_TRY(arc);
-            if (raw_out) B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_K5 + 1 + (r & 1)], c->copy_out));      // the read-back of this UOUT buffer
-            tail_len = avail - take; tail_ptr = UOUT + take;
         }
-        ubase_total += ulen_out; ilen_total += ilen_out;
+        B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_INDEX_FREE], c->copy_out));
+        const uint64_t avail = tail_len + ulen_out;
+        const uint64_t take = (r == nr - 1) ? avail : avail / L * L;
+        const uint64_t slice = std::max<uint64_t>(L, std::max<uint64_t>(512ull << 20, bytes_read / 32) / L * L);      // pieces of ~512 MiB keep the read-back close behind
+        for (uint64_t off = 0; off < take; off += slice) B200C_TRY(out_stream_append(os, UOUT + off, std::min(slice, take - off)));
+        if (raw_out) B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_UOUT_FREE + (r & 1)], c->copy_out));      // the read-back of this UOUT buffer
+        tail_len = avail - take; tail_ptr = UOUT + take;
+        return B200C_OK;
     }
-    // (progress: the last piece left bytes_scanned at (4 nr - 1) / (4 nr) of the input; the wrap-up below takes it to the total)
 
-    // ---- K5 wrap-up / remaining writers ------------------------------------------------------------------------------------------------
-    int rc = B200C_OK;
-    auto finish_common = [&](RunStats& rs) -> int {          // error word, stats, histogram, stage clock
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_err, 8, cudaMemcpyDeviceToHost, st));
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 8, d_stats, sizeof(RunStats), cudaMemcpyDeviceToHost, st));
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 16, d_hist, MAXK * 8, cudaMemcpyDeviceToHost, st));
-        B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 201, d_rbytes, 8, cudaMemcpyDeviceToHost, st));
+    // ---- the writers -------------------------------------------------------------------------------------------------------------------
+    int finish_common(RunStats& rs) {          // error word, stats, histogram, stage clock
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->err, d_err, 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(P->run_stats, d_stats, sizeof(RunStats), cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(P->hist, d_hist, MAXK * 8, cudaMemcpyDeviceToHost, st));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->bytes_in_range, d_rbytes, 8, cudaMemcpyDeviceToHost, st));
         mark(-1);
-        int trc = timing_end(c);
-        if (trc != B200C_OK) return trc;
+        B200C_TRY(timing_end(c));
         finish_marks();
-        if (h[0] != ~0ull) { c->err = "internal error: size/emit pass disagreement at output partition " + std::to_string(h[0] & 0xFFFFFFFFFFFFull); return B200C_ECUDA; }
-        memcpy(&rs, h + 8, sizeof(rs));
+        if (P->err != ~0ull) { c->err = "internal error: size/emit pass disagreement at output partition " + std::to_string(P->err & 0xFFFFFFFFFFFFull); return B200C_ECUDA; }
+        memcpy(&rs, P->run_stats, sizeof(rs));
         memset(res->merged_row_counts, 0, sizeof(res->merged_row_counts));
-        for (int k = 0; k < MAXK; k++) res->merged_row_counts[k] = h[16 + k];
-        res->bytes_read = bytes_read; res->bytes_in_range = h[201]; res->bytes_written = ubase_total; res->total_source_rows = rs.merged_unfiltereds + nparts_total /* one applyToStatic -> updateProgress per merged partition */; res->input_partitions = ncontrib_total;
+        for (int k = 0; k < MAXK; k++) res->merged_row_counts[k] = P->hist[k];
+        res->bytes_read = bytes_read; res->bytes_in_range = P->bytes_in_range; res->bytes_written = ubase_total; res->total_source_rows = rs.merged_unfiltereds + nparts_total /* one applyToStatic -> updateProgress per merged partition */; res->input_partitions = ncontrib_total;
         res->kernel_ms = c->last_ms; res->kernel_launches = c->launches_call;
         return B200C_OK;
-    };
+    }
+    struct FileOut { uint64_t data_len, index_len, nchunks, data_length; uint32_t digest; RunStats rs; };
+    static void describe(b200c_output& o, const FileOut& f) {
+        o.data_len = f.data_len; o.index_len = f.index_len; o.nchunks = f.nchunks; o.data_length = f.data_length; o.digest = f.digest; o.partitions = f.rs.partitions_out; o.rows = f.rs.rows_out;
+    }
+    // a written file goes to output slot o when it fits there (fits: and it was not found too large already): Data.db from `data` (nullptr:
+    // K5 wrote it there), Index.db from `index` (nullptr: it went out piece by piece), the chunk offsets. Otherwise the call returns
+    // B200C_ETOOSMALL once it has run to its end. *done: whether it went out.
+    int publish(const b200c_output& o, const FileOut& f, bool fits, const uint8_t* data, const uint8_t* index, const uint64_t* d_offs, cudaMemcpyKind kind, bool* done = nullptr) {
+        fits = fits && f.data_len <= o.data_cap && f.index_len <= o.index_cap && f.nchunks <= o.chunk_cap;
+        if (done) *done = fits;
+        if (!fits) { c->err = "output buffers too small"; rc = B200C_ETOOSMALL; return B200C_OK; }
+        if (data && f.data_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(o.data, data, f.data_len, kind, st));
+        if (index && f.index_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(o.index, index, f.index_len, kind, st));
+        if (f.nchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(o.chunk_offsets, d_offs, f.nchunks * 8, kind, st));
+        B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
+        return B200C_OK;
+    }
+    // the single output file: its sizes, its side band (which still goes out when the file does not fit), then the file
+    int publish_single(const FileOut& f, bool fits, const uint8_t* index, const uint64_t* d_offs, cudaMemcpyKind kind) {
+        b200c_output& out = res->outputs[0];
+        res->noutputs = 1;
+        describe(out, f);
+        { const int mrc = finish_meta(out); if (mrc != B200C_OK) rc = mrc; }
+        return publish(out, f, fits, nullptr, index, d_offs, kind);
+    }
     // Filter.db / Summary.db / first+last key / statistics side band of the single output -> the caller's (host) buffers
-    auto finish_meta = [&](b200c_output& out) -> int {
+    int finish_meta(b200c_output& out) {
         if (!want_meta) return B200C_OK;
         TdropDense* d_tdd; B200C_TRY(ws_typed(c, WS_META_TDD, 1, &d_tdd));
         B200C_CUDA_TRY(c, cudaMemsetAsync(d_tdd, 0, 8, st));
@@ -1985,8 +2008,8 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
             if (out.summary_len > out.summary_cap) { c->err = "summary buffer too small"; return B200C_ETOOSMALL; }
             if (written_total) {
                 uint8_t* p = out.summary;
-                auto be32 = [&](uint32_t v) { *p++ = (uint8_t)(v >> 24); *p++ = (uint8_t)(v >> 16); *p++ = (uint8_t)(v >> 8); *p++ = (uint8_t)v; };
-                auto be64 = [&](uint64_t v) { be32((uint32_t)(v >> 32)); be32((uint32_t)v); };
+                auto be32 = [&p](uint32_t v) { *p++ = (uint8_t)(v >> 24); *p++ = (uint8_t)(v >> 16); *p++ = (uint8_t)(v >> 8); *p++ = (uint8_t)v; };
+                auto be64 = [&be32](uint64_t v) { be32((uint32_t)(v >> 32)); be32((uint32_t)v); };
                 be32(meta_interval); be32((uint32_t)n); be64(4 * n + eb); be32(128); be32((uint32_t)((written_total + meta_interval - 1) / meta_interval));
                 std::vector<uint64_t> offs(n);
                 if (n) B200C_CUDA_TRY(c, cudaMemcpyAsync(offs.data(), d_sumoff, n * 8, cudaMemcpyDeviceToHost, st));
@@ -2016,59 +2039,71 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         }
         B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
         return B200C_OK;
-    };
-    if (to_host_stream) {
-        b200c_output& out = out0;
+    }
+    // one output file in host memory: K5 streamed it out piece by piece
+    int write_host_stream() {
         uint64_t out_len = 0; uint32_t digest = 0; uint64_t* d_ooffs = nullptr;
-        if (k5_last >= 0) B200C_CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_pool[k5_last], 0));      // every piece's K5 is done before the digest
         B200C_TRY(out_stream_finish(os, &out_len, &digest, &d_ooffs));
-        const uint64_t nchunks_out = os.nchunks;
         RunStats rs; B200C_TRY(finish_common(rs));
-        res->noutputs = 1;
-        res->required_data_cap = std::max<uint64_t>(out_len, 1); res->required_index_cap = ilen_total; res->required_chunk_cap = nchunks_out;
-        out.data_len = out_len; out.index_len = ilen_total; out.nchunks = nchunks_out; out.data_length = ubase_total; out.digest = digest;
-        out.partitions = rs.partitions_out; out.rows = rs.rows_out;
-        { int mrc = finish_meta(out); if (mrc != B200C_OK) rc = mrc; }
-        if (!os.fits || !index_fits || out_len > out.data_cap || ilen_total > out.index_cap || nchunks_out > out.chunk_cap) { c->err = "output buffers too small"; rc = B200C_ETOOSMALL; }
-        else {
-            if (nchunks_out) B200C_CUDA_TRY(c, cudaMemcpyAsync(out.chunk_offsets, d_ooffs, nchunks_out * 8, cudaMemcpyDeviceToHost, st));
-            B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-        }
+        res->required_data_cap = std::max<uint64_t>(out_len, 1); res->required_index_cap = ilen_total; res->required_chunk_cap = os.nchunks;
+        B200C_TRY(publish_single(FileOut{out_len, ilen_total, os.nchunks, ubase_total, digest, rs}, os.fits && index_fits, nullptr, d_ooffs, cudaMemcpyDeviceToHost));
         B200C_CUDA_TRY(c, cudaStreamSynchronize(c->copy_out));
-    } else if (!lcs) {
-        // one output file in device memory
-        b200c_output& out = out0;
+        return B200C_OK;
+    }
+    // one output file in device memory
+    int write_device() {
+        b200c_output& out = res->outputs[0];
         const uint64_t nchunks_out = (ulen_out + L - 1) / L;
         const uint64_t bound = b200c_compress_bound(m->out_compressor, ulen_out, m->out_chunk_len);
         res->required_data_cap = bound; res->required_index_cap = ilen_out; res->required_chunk_cap = nchunks_out;
-        if (out.data_cap < bound) { c->err = "output data buffer too small"; timing_end(c); return B200C_ETOOSMALL; }
+        if (out.data_cap < bound) { c->err = "output data buffer too small"; return B200C_ETOOSMALL; }
         uint64_t* d_ooffs; B200C_TRY(ws_typed(c, WS_OOFFS, nchunks_out + 2, &d_ooffs));
         uint64_t out_len = 0; uint32_t digest = 0;
         if (raw_out) { B200C_TRY(raw_stream_device(c, UOUT, ulen_out, m->out_chunk_len, out.data, d_ooffs, &digest, WS_CODEC)); out_len = ulen_out; }
         else B200C_TRY(compress_stream_device(c, m->out_compressor, UOUT, ulen_out, m->out_chunk_len, m->out_max_compressed_len, out.data, bound, d_ooffs, &out_len, &digest, WS_CODEC));
         RunStats rs; B200C_TRY(finish_common(rs));
-        res->noutputs = 1;
-        out.data_len = out_len; out.index_len = ilen_out; out.nchunks = nchunks_out; out.data_length = ulen_out; out.digest = digest;
-        out.partitions = rs.partitions_out; out.rows = rs.rows_out;
-        { int mrc = finish_meta(out); if (mrc != B200C_OK) rc = mrc; }
-        if (out_len > out.data_cap || ilen_out > out.index_cap || nchunks_out > out.chunk_cap) { c->err = "output buffers too small"; rc = B200C_ETOOSMALL; }
-        else {
-            if (ilen_out) B200C_CUDA_TRY(c, cudaMemcpyAsync(out.index, IOUT, ilen_out, cudaMemcpyDeviceToDevice, st));
-            if (nchunks_out) B200C_CUDA_TRY(c, cudaMemcpyAsync(out.chunk_offsets, d_ooffs, nchunks_out * 8, cudaMemcpyDeviceToDevice, st));
+        return publish_single(FileOut{out_len, ilen_out, nchunks_out, ulen_out, digest, rs}, true, IOUT, d_ooffs, cudaMemcpyDeviceToDevice);
+    }
+    // multi-file output, the next file starting at partition jlo, byte start_b of the merged stream: jhi = its first partition after it,
+    // done = chunks of the rest compressed so far into slots. How much to compress before looking for the file boundary: the file holds
+    // max_sstable_bytes of COMPRESSED chunks, so the window is that divided by the ratio seen so far plus 8 %; a window that turns out too
+    // short is extended (doubling), nothing is compressed twice. An uncompressed output cuts at the exact position (k_find_cut_raw).
+    int lcs_cut(uint64_t jlo, uint64_t start_b, double est_ratio, uint64_t& jhi, uint64_t& done) {
+        const uint64_t remaining = ulen_out - start_b, rem_chunks = (remaining + L - 1) / L;
+        uint64_t want = 0, status = raw_out ? 0 : 2; jhi = nparts; done = 0;
+        if (raw_out) {
+            B200C_LAUNCH(c, k_find_cut_raw, 1, 1, 0, d_dpos, jlo, nparts, start_b, m->max_sstable_bytes, d_cut);
+            B200C_CUDA_TRY(c, cudaMemcpyAsync(P->cut, d_cut, 8, cudaMemcpyDeviceToHost, st));
             B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
+            jhi = P->cut[0];
+        } else want = std::max<uint64_t>(64, (uint64_t)((double)m->max_sstable_bytes / est_ratio * 1.08) / L + 8);
+        while (status == 2) {
+            uint64_t W = std::min(rem_chunks, want);
+            if (W > done) B200C_TRY(compress_slots_device(c, m->out_compressor, UOUT + start_b + done * L, std::min(remaining - done * L, (W - done) * (uint64_t)L), (int)L,
+                                                          m->out_max_compressed_len, slots + done * lcs_stride, lcs_stride, file_len + done, seg_raw + done));
+            done = W;
+            // bytes flushed before a partition = whole chunks only: a trailing partial chunk of the window is not "flushed"
+            uint64_t nfull_known = (W == rem_chunks) ? (remaining / L) : W;
+            B200C_TRY(exclusive_scan<uint32_t>(c, file_len, nfull_known, woffs, WS_SCANA, 0));
+            B200C_LAUNCH(c, k_find_cut, 1, 1, 0, d_dpos, jlo, nparts, start_b, woffs, (W == rem_chunks) ? ~0ull >> 1 : nfull_known, L, m->max_sstable_bytes, d_cut);
+            B200C_CUDA_TRY(c, cudaMemcpyAsync(P->cut, d_cut, 16, cudaMemcpyDeviceToHost, st));
+            B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
+            jhi = P->cut[0]; status = P->cut[1];
+            if (status == 2) { if (W == rem_chunks) { status = 1; jhi = nparts; } else want *= 2; }
         }
-    } else {
-        // ---- multi-file output: one pass per file over a compressed window (see k_find_cut) ----------------------------------------
-        const int comp = m->out_compressor; const int stride = chunk_slot_stride(comp, (int)L);
+        return B200C_OK;
+    }
+    // ---- multi-file output: one pass per file over a compressed window (see k_find_cut) ----------------------------------------------
+    int write_lcs() {
+        const int comp = m->out_compressor; lcs_stride = chunk_slot_stride(comp, (int)L);
         const uint64_t nch_total = (ulen_out + L - 1) / L;
-        uint64_t *woffs = nullptr, *d_dposf, *d_iposf, *d_cut, *d_ooffs; uint8_t* IOUTF; RunStats* d_fstats;
-        uint8_t* slots = nullptr; uint32_t *file_len = nullptr, *seg_raw = nullptr; uint8_t* d_dout = nullptr;      // (compressed output only)
+        uint64_t *d_dposf, *d_iposf, *d_ooffs; uint8_t *IOUTF, *d_dout = nullptr; RunStats* d_fstats;
         if (!raw_out) {
-            B200C_TRY(ws_typed(c, WS_CODEC + 2, (nch_total + 2) * (uint64_t)stride, &slots));
+            B200C_TRY(ws_typed(c, WS_CODEC + 2, (nch_total + 2) * (uint64_t)lcs_stride, &slots));
             B200C_TRY(ws_typed(c, WS_CODEC + 3, nch_total + 2, &file_len));
             B200C_TRY(ws_typed(c, WS_CODEC + 4, nch_total + 2, &seg_raw));
+            B200C_TRY(ws_typed(c, WS_LCS0, nch_total + 4, &woffs));
         }
-        if (!raw_out) B200C_TRY(ws_typed(c, WS_LCS0, nch_total + 4, &woffs));
         B200C_TRY(ws_typed(c, WS_LCS1, nparts + 2, &d_dposf));
         B200C_TRY(ws_typed(c, WS_LCS2, nparts + 2, &d_iposf));
         B200C_TRY(ws_typed(c, WS_LCS3, 64, &d_cut)); d_fstats = (RunStats*)(d_cut + 8);
@@ -2079,45 +2114,22 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         if (!raw_out) B200C_TRY(ws_typed(c, WS_DOUT, file_bound + 64, &d_dout));
         res->required_data_cap = res->required_index_cap = res->required_chunk_cap = 0;
         uint64_t jlo = 0, start_b = 0; int f = 0;
-        // how much of the stream to compress before looking for the file boundary: the file holds max_sstable_bytes of COMPRESSED chunks, so the
-        // window is that divided by the ratio seen so far (the inputs' own ratio for the first file, then the previous file's) plus 8 %; a window
-        // that turns out too short is extended below (doubling), nothing is compressed twice
-        double est_ratio = 0.5;
+        double est_ratio = 0.5;                    // the inputs' own ratio for the first file, then the previous file's
         if (!raw_out) { uint64_t ci = 0, ui = 0; for (int i = 0; i < K; i++) { ci += m->inputs[i].data_len; ui += m->inputs[i].data_length; } if (ui) est_ratio = std::min(1.0, std::max(0.05, (double)ci / (double)ui)); }
         while (jlo < nparts && start_b < ulen_out) {
             B200C_TRY(check_cancel());
-            const uint64_t remaining = ulen_out - start_b, rem_chunks = (remaining + L - 1) / L;
-            uint64_t want = 0, done = 0, jhi = nparts, status = raw_out ? 0 : 2;
-            if (raw_out) {                                   // the exact position decides (k_find_cut_raw): nothing to compress first
-                B200C_LAUNCH(c, k_find_cut_raw, 1, 1, 0, d_dpos, jlo, nparts, start_b, m->max_sstable_bytes, d_cut);
-                B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_cut, 8, cudaMemcpyDeviceToHost, st));
-                B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-                jhi = h[0];
-            } else want = std::max<uint64_t>(64, (uint64_t)((double)m->max_sstable_bytes / est_ratio * 1.08) / L + 8);
-            while (status == 2) {
-                uint64_t W = std::min(rem_chunks, want);
-                if (W > done) B200C_TRY(compress_slots_device(c, comp, UOUT + start_b + done * L, std::min(remaining - done * L, (W - done) * (uint64_t)L), (int)L,
-                                                              m->out_max_compressed_len, slots + done * stride, stride, file_len + done, seg_raw + done));
-                done = W;
-                // bytes flushed before a partition = whole chunks only: a trailing partial chunk of the window is not "flushed"
-                uint64_t nfull_known = (W == rem_chunks) ? (remaining / L) : W;
-                B200C_TRY(exclusive_scan<uint32_t>(c, file_len, nfull_known, woffs, WS_SCANA, 0));
-                B200C_LAUNCH(c, k_find_cut, 1, 1, 0, d_dpos, jlo, nparts, start_b, woffs, (W == rem_chunks) ? ~0ull >> 1 : nfull_known, L, m->max_sstable_bytes, d_cut);
-                B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_cut, 16, cudaMemcpyDeviceToHost, st));
-                B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-                jhi = h[0]; status = h[1];
-                if (status == 2) { if (W == rem_chunks) { status = 1; jhi = nparts; } else want *= 2; }
-            }
+            uint64_t jhi, done;
+            B200C_TRY(lcs_cut(jlo, start_b, est_ratio, jhi, done));
             // the file is partitions [jlo, jhi), bytes [start_b, end_b)
             uint64_t end_b = ulen_out;
-            if (jhi < nparts) { B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_dpos + jhi, 8, cudaMemcpyDeviceToHost, st)); B200C_CUDA_TRY(c, cudaStreamSynchronize(st)); end_b = h[0]; }
+            if (jhi < nparts) { B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->file_end, d_dpos + jhi, 8, cudaMemcpyDeviceToHost, st)); B200C_CUDA_TRY(c, cudaStreamSynchronize(st)); end_b = P->file_end; }
             const uint64_t flen = end_b - start_b, fchunks = (flen + L - 1) / L, nfull = flen / L, tail = flen % L;
             uint64_t out_len = 0; uint32_t digest = 0;
             if (raw_out) { B200C_TRY(raw_stream_device(c, UOUT + start_b, flen, (int)L, nullptr, d_ooffs, &digest, WS_CODEC)); out_len = flen; }
             else {
-                if (tail && !(end_b == ulen_out && done == rem_chunks))      // the last chunk of the file is shorter than what the window compressed there
-                    B200C_TRY(compress_slots_device(c, comp, UOUT + start_b + nfull * L, tail, (int)L, m->out_max_compressed_len, slots + nfull * stride, stride, file_len + nfull, seg_raw + nfull));
-                B200C_TRY(pack_digest_device(c, slots, stride, file_len, seg_raw, fchunks, d_dout, file_bound, d_ooffs, &out_len, &digest, WS_CODEC));
+                if (tail && !(end_b == ulen_out && done == (ulen_out - start_b + L - 1) / L))      // the last chunk of the file is shorter than what the window compressed there
+                    B200C_TRY(compress_slots_device(c, comp, UOUT + start_b + nfull * L, tail, (int)L, m->out_max_compressed_len, slots + nfull * lcs_stride, lcs_stride, file_len + nfull, seg_raw + nfull));
+                B200C_TRY(pack_digest_device(c, slots, lcs_stride, file_len, seg_raw, fchunks, d_dout, file_bound, d_ooffs, &out_len, &digest, WS_CODEC));
             }
             // Index.db of this file: positions relative to the file start
             const uint64_t cnt = jhi - jlo;
@@ -2132,28 +2144,20 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
                                         d_nblk + jlo, d_ovf + jlo, d_ihead + jlo, d_ipay + jlo, d_iposf + jlo, d_ioff + jlo, d_icap + jlo, ISCR, IOUTF);
             ka.dbase = UOUT + start_b; ka.iout = IOUTF; ka.dpos = d_dposf; ka.ipos = d_iposf; ka.jlo = jlo; ka.jhi = jhi;
             B200C_TRY(launch_k4(3));
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_iposf + jhi, 8, cudaMemcpyDeviceToHost, st));
-            B200C_CUDA_TRY(c, cudaMemcpyAsync(h + 8, d_fstats, sizeof(RunStats), cudaMemcpyDeviceToHost, st));
+            B200C_CUDA_TRY(c, cudaMemcpyAsync(&P->file_index_len, d_iposf + jhi, 8, cudaMemcpyDeviceToHost, st));
+            B200C_CUDA_TRY(c, cudaMemcpyAsync(P->file_stats, d_fstats, sizeof(RunStats), cudaMemcpyDeviceToHost, st));
             B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-            const uint64_t filen = h[0]; RunStats fs; memcpy(&fs, h + 8, sizeof(fs));
+            FileOut fo{out_len, P->file_index_len, fchunks, flen, digest, {}}; memcpy(&fo.rs, P->file_stats, sizeof(fo.rs));
             if (flen && out_len) est_ratio = std::min(1.0, std::max(0.05, (double)out_len / (double)flen));
             res->required_data_cap = std::max<uint64_t>(res->required_data_cap, out_len);
-            res->required_index_cap = std::max<uint64_t>(res->required_index_cap, filen);
+            res->required_index_cap = std::max<uint64_t>(res->required_index_cap, fo.index_len);
             res->required_chunk_cap = std::max<uint64_t>(res->required_chunk_cap, fchunks);
-            if (fs.partitions_out) {
+            if (fo.rs.partitions_out) {
                 if (f >= res->noutputs_cap) { c->err = "more output files than output slots"; rc = B200C_ETOOSMALL; }
                 else {
-                    b200c_output& o = res->outputs[f];
-                    if (out_len > o.data_cap || filen > o.index_cap || fchunks > o.chunk_cap) { c->err = "output buffers too small"; rc = B200C_ETOOSMALL; }
-                    else {
-                        cudaMemcpyKind k = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-                        if (out_len) B200C_CUDA_TRY(c, cudaMemcpyAsync(o.data, raw_out ? UOUT + start_b : d_dout, out_len, k, st));
-                        if (filen) B200C_CUDA_TRY(c, cudaMemcpyAsync(o.index, IOUTF, filen, k, st));
-                        if (fchunks) B200C_CUDA_TRY(c, cudaMemcpyAsync(o.chunk_offsets, d_ooffs, fchunks * 8, k, st));
-                        B200C_CUDA_TRY(c, cudaStreamSynchronize(st));
-                        o.data_len = out_len; o.index_len = filen; o.nchunks = fchunks; o.data_length = flen; o.digest = digest;
-                        o.partitions = fs.partitions_out; o.rows = fs.rows_out;
-                    }
+                    bool sent;
+                    B200C_TRY(publish(res->outputs[f], fo, true, raw_out ? UOUT + start_b : d_dout, IOUTF, d_ooffs, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, &sent));
+                    if (sent) describe(res->outputs[f], fo);
                 }
                 f++;
             }
@@ -2161,10 +2165,33 @@ int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int 
         }
         RunStats rs; B200C_TRY(finish_common(rs));
         res->noutputs = f;
+        return B200C_OK;
     }
-    c->prog_scanned.store(bytes_read); c->prog_stage.store(6);
-    res->total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
-    return rc;
+};
+
+} // namespace
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+extern "C" {
+
+int b200c_compact(b200c_ctx* c, const b200c_manifest* m, b200c_result* res, int flags) {
+    if (!c || !m || !res) return B200C_EINVAL;
+    CompactCall call(c, m, res, flags);
+    B200C_TRY(call.validate());
+    B200C_TRY(call.plan_slices());
+    B200C_TRY(call.layout());
+    call.plan_pieces();
+    B200C_TRY(call.workspace());
+    B200C_TRY(call.stage_inputs());
+    B200C_TRY(call.k1_inputs());
+    B200C_TRY(call.k2_inputs());
+    B200C_TRY(call.begin_output());
+    for (int r = 0; r < call.nr; r++) B200C_TRY(call.piece(r));
+    // (progress: the last piece left bytes_scanned at (4 nr - 1) / (4 nr) of the input; the end of the call takes it to the total)
+    B200C_TRY(call.to_host_stream ? call.write_host_stream() : !call.lcs ? call.write_device() : call.write_lcs());
+    c->prog_scanned.store(call.bytes_read); c->prog_stage.store(6);
+    res->total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - call.t_start).count();
+    return call.rc;
 }
 
 int64_t b200c_token(int partitioner, const uint8_t* key, uint32_t len) {

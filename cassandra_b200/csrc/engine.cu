@@ -108,7 +108,7 @@ int pack_digest_device(b200c_ctx* c, const uint8_t* slots, int stride, const uin
     uint32_t* acc; B200C_TRY(ws_typed(c, ws_base + WSC_ACC, 4, &acc));
     B200C_CUDA_TRY(c, cudaMemsetAsync(acc, 0, 16, c->stream));
     B200C_TRY(exclusive_scan<uint32_t>(c, file_len, nchunks, d_offs, ws_base + WSC_SCAN0, 0));
-    uint64_t* h = (uint64_t*)c->h_pinned;                 // the total size must be known on the host before packing into the caller's buffer
+    uint64_t* h = &c->h_pinned->packed_len;               // the total size must be known on the host before packing into the caller's buffer
     B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_offs + nchunks, 8, cudaMemcpyDeviceToHost, c->stream));
     B200C_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     *out_len = h[0];
@@ -116,7 +116,7 @@ int pack_digest_device(b200c_ctx* c, const uint8_t* slots, int stride, const uin
     B200C_LAUNCH(c, k_pack_chunks, (unsigned)((nchunks + 3) / 4), 128, 0, slots, stride, file_len, d_offs, nchunks, d_out, (const uint64_t*)nullptr);
     B200C_LAUNCH(c, k_digest, (unsigned)((nchunks + 255) / 256), 256, 0, c->d_tables, seg_raw, d_offs, nchunks, acc);
     B200C_LAUNCH(c, k_digest_final, 1, 1, 0, c->d_tables, d_offs, nchunks, acc);
-    uint32_t* h32 = (uint32_t*)c->h_pinned;
+    uint32_t* h32 = &c->h_pinned->digest;
     B200C_CUDA_TRY(c, cudaMemcpyAsync(h32, acc + 1, 4, cudaMemcpyDeviceToHost, c->stream));
     B200C_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     *digest = h32[0];
@@ -161,16 +161,16 @@ int out_stream_begin(OutStream& o, b200c_ctx* c, int comp, int chunk_len, int ma
 
 static int out_stream_drain(OutStream& o, int s) {       // piece s is packed once its event fires: hand its bytes to the copy engine
     b200c_ctx* c = o.c;
-    uint64_t* h = (uint64_t*)c->h_pinned + 1024;
-    B200C_CUDA_TRY(c, cudaEventSynchronize(c->ev_pool[2 * s]));
+    uint64_t* h = c->h_pinned->os_end;
+    B200C_CUDA_TRY(c, cudaEventSynchronize(c->ev_pool[EV_OUT_PIECE + 2 * s]));
     const uint64_t end = h[s];
     if (end - o.copied > o.img_cap[s & 1]) { c->err = "internal error: compressed piece exceeds its bound"; return B200C_ECUDA; }
     if (end > o.h_cap) o.fits = false;
     if (o.fits && end > o.copied) {
-        B200C_CUDA_TRY(c, cudaStreamWaitEvent(c->copy_out, c->ev_pool[2 * s], 0));
+        B200C_CUDA_TRY(c, cudaStreamWaitEvent(c->copy_out, c->ev_pool[EV_OUT_PIECE + 2 * s], 0));
         B200C_CUDA_TRY(c, cudaMemcpyAsync(o.h_out + o.copied, o.img[s & 1], end - o.copied, cudaMemcpyDeviceToHost, c->copy_out));
     }
-    B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[2 * s + 1], c->copy_out));
+    B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_OUT_PIECE + 2 * s + 1], c->copy_out));
     o.copied = end;
     return B200C_OK;
 }
@@ -193,10 +193,10 @@ int out_stream_append(OutStream& o, const uint8_t* d_in, uint64_t nbytes) {
         RawArgs ra; memset(&ra, 0, sizeof(ra));
         ra.src = d_in; ra.n = nbytes; ra.L = o.L; ra.chunk_end = k; ra.crc_out = o.d_offs + a; ra.seg_raw = o.seg_raw + a; ra.ends = o.ends + a; ra.ebase = o.ulen;
         B200C_TRY(raw_chunks_device(c, false, ra));
-        B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[2 * s], c->stream));
+        B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_OUT_PIECE + 2 * s], c->stream));
         if (o.ulen + nbytes > o.h_cap) o.fits = false;
         if (o.fits) {
-            B200C_CUDA_TRY(c, cudaStreamWaitEvent(c->copy_out, c->ev_pool[2 * s], 0));
+            B200C_CUDA_TRY(c, cudaStreamWaitEvent(c->copy_out, c->ev_pool[EV_OUT_PIECE + 2 * s], 0));
             B200C_CUDA_TRY(c, cudaMemcpyAsync(o.h_out + o.ulen, d_in, nbytes, cudaMemcpyDeviceToHost, c->copy_out));
         }
         o.nchunks += k; o.ulen += nbytes; o.copied = o.ulen; o.piece++;
@@ -210,14 +210,13 @@ int out_stream_append(OutStream& o, const uint8_t* d_in, uint64_t nbytes) {
     B200C_TRY(ws_typed(c, o.ws_base + WSC_IN, k + 2, &rel));
     B200C_TRY(ws_typed(c, o.ws_base + (s & 1 ? WSC_OUT : WSC_ERR), k * (uint64_t)o.stride + 64, &o.img[s & 1]));
     o.img_cap[s & 1] = k * (uint64_t)o.stride;
-    if (s >= 2) B200C_CUDA_TRY(c, cudaStreamWaitEvent(c->stream, c->ev_pool[2 * (s - 2) + 1], 0));   // the image buffer is free again
+    if (s >= 2) B200C_CUDA_TRY(c, cudaStreamWaitEvent(c->stream, c->ev_pool[EV_OUT_PIECE + 2 * (s - 2) + 1], 0));   // the image buffer is free again
     B200C_TRY(compress_slots_device(c, o.comp, d_in, nbytes, o.L, o.max_clen, slots, o.stride, o.file_len + a, o.seg_raw + a));
     B200C_TRY(exclusive_scan<uint32_t>(c, o.file_len + a, k, rel, o.ws_base + WSC_SCAN0, 0));
     B200C_LAUNCH(c, k_offs_add_base, (unsigned)((k + 1 + 255) / 256), 256, 0, rel, k, o.bases + s, o.d_offs + a);
     B200C_LAUNCH(c, k_pack_chunks, (unsigned)((k + 3) / 4), 128, 0, slots, o.stride, o.file_len + a, o.d_offs + a, k, o.img[s & 1], (const uint64_t*)(o.bases + s));
-    uint64_t* h = (uint64_t*)c->h_pinned + 1024;
-    B200C_CUDA_TRY(c, cudaMemcpyAsync(h + s, o.bases + s + 1, 8, cudaMemcpyDeviceToHost, c->stream));
-    B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[2 * s], c->stream));
+    B200C_CUDA_TRY(c, cudaMemcpyAsync(c->h_pinned->os_end + s, o.bases + s + 1, 8, cudaMemcpyDeviceToHost, c->stream));
+    B200C_CUDA_TRY(c, cudaEventRecord(c->ev_pool[EV_OUT_PIECE + 2 * s], c->stream));
     if (s) B200C_TRY(out_stream_drain(o, s - 1));        // after piece s is queued, so the GPU never waits for the host
     o.nchunks += k; o.ulen += nbytes; o.piece++;
     return B200C_OK;
@@ -234,7 +233,7 @@ int out_stream_finish(OutStream& o, uint64_t* out_len, uint32_t* digest, uint64_
         *out_len = o.ulen; *d_offs_out = o.d_offs;
         return B200C_OK;
     }
-    uint32_t* h32 = (uint32_t*)((uint64_t*)c->h_pinned + 1024 + OutStream::MAX_PIECES + 1);
+    uint32_t* h32 = &c->h_pinned->os_digest;
     B200C_LAUNCH(c, k_digest, (unsigned)((o.nchunks + 255) / 256), 256, 0, c->d_tables, o.seg_raw, o.d_offs, o.nchunks, o.acc);
     B200C_LAUNCH(c, k_digest_final, 1, 1, 0, c->d_tables, o.d_offs, o.nchunks, o.acc);
     B200C_CUDA_TRY(c, cudaMemcpyAsync(h32, o.acc + 1, 4, cudaMemcpyDeviceToHost, c->stream));
@@ -333,7 +332,7 @@ int raw_chunks_device(b200c_ctx* c, bool ingest, const RawArgs& a) {
 static int raw_digest(b200c_ctx* c, const uint32_t* seg_raw, const uint64_t* ends, uint64_t nchunks, uint32_t* acc, uint32_t* digest) {
     B200C_LAUNCH(c, k_digest, (unsigned)((nchunks + 255) / 256), 256, 0, c->d_tables, seg_raw, ends, nchunks, acc);
     B200C_LAUNCH(c, k_digest_final, 1, 1, 0, c->d_tables, ends, nchunks, acc);
-    uint32_t* h32 = (uint32_t*)c->h_pinned;
+    uint32_t* h32 = &c->h_pinned->digest;
     B200C_CUDA_TRY(c, cudaMemcpyAsync(h32, acc + 1, 4, cudaMemcpyDeviceToHost, c->stream));
     B200C_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     *digest = h32[0];
@@ -384,13 +383,11 @@ b200c_ctx* b200c_create(int device, size_t workspace_bytes) {
     for (auto& e : c->ev_in) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
     for (auto& e : c->ev_pool) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
     cudaStreamCreateWithFlags(&c->copy_out, cudaStreamNonBlocking);
-    cudaStreamCreateWithFlags(&c->stream5, cudaStreamNonBlocking);
     DevTables* h = new DevTables(); build_tables(h);
     if (cudaMalloc(&c->d_tables, sizeof(DevTables)) != cudaSuccess) { delete h; delete c; return nullptr; }
     cudaMemcpy(c->d_tables, h, sizeof(DevTables), cudaMemcpyHostToDevice);
     delete h;
-    c->h_pinned_cap = 1 << 16;
-    if (cudaMallocHost(&c->h_pinned, c->h_pinned_cap) != cudaSuccess) { cudaFree(c->d_tables); delete c; return nullptr; }
+    if (cudaMallocHost((void**)&c->h_pinned, H_PINNED_CAP) != cudaSuccess) { cudaFree(c->d_tables); delete c; return nullptr; }
     cudaFuncSetAttribute(k_compress_chunks, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536 + 65536 + 16);
     cudaFuncSetAttribute(k_compress_chunks_snappy_direct, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536);
     k1_plan(c);
@@ -410,8 +407,6 @@ void b200c_destroy(b200c_ctx* c) {
     for (auto& e : c->ev_in) cudaEventDestroy(e);
     for (auto& e : c->ev_pool) cudaEventDestroy(e);
     for (auto& e : c->ev_marks) cudaEventDestroy(e);
-    if (c->stream5) cudaStreamDestroy(c->stream5);
-    for (auto e : c->ev_k5) cudaEventDestroy(e);
     if (c->copy_out) cudaStreamDestroy(c->copy_out);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     cudaStreamDestroy(c->stream);
@@ -539,7 +534,7 @@ int b200c_decompress_chunks(b200c_ctx* c, int comp, const uint8_t* data, uint64_
         int rc2 = timing_end(c);
         if (rc != B200C_OK) return rc;
         if (rc2 != B200C_OK) return rc2;
-        ChunkErr* h = (ChunkErr*)c->h_pinned;
+        ChunkErr* h = (ChunkErr*)&c->h_pinned->chunk_err;
         B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_err, sizeof(ChunkErr), cudaMemcpyDeviceToHost, c->stream));
         B200C_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
         if (h->first_bad != ~0ull) {
@@ -569,7 +564,7 @@ int b200c_decompress_chunks(b200c_ctx* c, int comp, const uint8_t* data, uint64_
     int rc2 = timing_end(c);
     if (rc != B200C_OK) return rc;
     if (rc2 != B200C_OK) return rc2;
-    ChunkErr* h = (ChunkErr*)c->h_pinned;
+    ChunkErr* h = (ChunkErr*)&c->h_pinned->chunk_err;
     B200C_CUDA_TRY(c, cudaMemcpyAsync(h, d_err, sizeof(ChunkErr), cudaMemcpyDeviceToHost, c->stream));
     B200C_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     if (h->first_bad != ~0ull) {

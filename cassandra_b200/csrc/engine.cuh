@@ -15,6 +15,13 @@ enum { WS_SLOTS = 160, WS_K5_ENT = 150, WS_K1_REC = 151, WS_K1_NSEQ = 152 };    
 
 struct WsBuf { void* p = nullptr; size_t cap = 0; };
 
+enum { MAX_RANGES = 16 };                // token-range pieces of one b200c_compact call
+// slots of b200c_ctx::ev_pool: OutStream piece s uses EV_OUT_PIECE + 2 s (packed) and + 2 s + 1 (copied out); b200c_compact uses
+// EV_RANGE + r (piece r's inputs are on the device), EV_INDEX_READY / EV_INDEX_FREE (a piece's Index.db is final / has left IOUT) and
+// EV_UOUT_FREE + (r & 1) (the merged stream of an uncompressed host output has left its buffer)
+enum { EV_OUT_PIECE = 0, EV_RANGE = 200, EV_INDEX_FREE = 220, EV_INDEX_READY = 221, EV_UOUT_FREE = 230, EV_POOL = 256 };
+struct Pinned;
+
 } // namespace b200c
 
 struct b200c_ctx {
@@ -27,7 +34,7 @@ struct b200c_ctx {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     b200c::DevTables* d_tables = nullptr;
     b200c::WsBuf ws[b200c::WS_SLOTS];
-    void* h_pinned = nullptr; size_t h_pinned_cap = 0;      // small pinned scratch for scalar read-backs
+    b200c::Pinned* h_pinned = nullptr;             // small pinned scratch for scalar read-backs
     std::string err;
     uint64_t launches_call = 0, launches_total = 0;
     double last_ms = 0.0;
@@ -44,10 +51,8 @@ struct b200c_ctx {
     cudaStream_t copy_stream = nullptr;            // host->device staging of the inputs, overlapped with K1 input by input
     cudaEvent_t ev_in[64] = {};
     std::vector<cudaEvent_t> ev_marks;             // timed events of the stage clock (grown on demand)
-    cudaEvent_t ev_pool[256] = {};                 // untimed events: OutStream pieces (2 each), token-range staging
+    cudaEvent_t ev_pool[b200c::EV_POOL] = {};      // untimed events (b200c::EV_*)
     cudaStream_t copy_out = nullptr;               // device->host stream of the outputs (the other copy engine)
-    cudaStream_t stream5 = nullptr;                // K5 of streamed piece r runs here, under K1..K3 (and the copies they wait for) of piece r + 1
-    std::vector<cudaEvent_t> ev_k5;                // timed event pairs around each piece's K5 on stream5 (stage clock)
 };
 
 namespace b200c {
@@ -78,7 +83,7 @@ inline int ws_get(b200c_ctx* c, int slot, size_t bytes, void** out) {
     return B200C_OK;
 }
 template <typename T> inline int ws_typed(b200c_ctx* c, int slot, size_t count, T** out) {
-    void* p; int rc = ws_get(c, slot, count * sizeof(T), &p); *out = (T*)p; return rc;
+    void* p = nullptr; int rc = ws_get(c, slot, count * sizeof(T), &p); *out = (T*)p; return rc;
 }
 
 // workspace slot that keeps its first `used` bytes when it has to grow (whole-file arrays of an OutStream)
@@ -119,6 +124,36 @@ struct OutStream {
 int out_stream_begin(OutStream& o, b200c_ctx* c, int comp, int chunk_len, int max_clen, uint8_t* h_out, uint64_t h_cap, int ws_base);
 int out_stream_append(OutStream& o, const uint8_t* d_in, uint64_t nbytes);
 int out_stream_finish(OutStream& o, uint64_t* out_len, uint32_t* digest, uint64_t** d_offs_out);
+
+static_assert(EV_OUT_PIECE + 2 * OutStream::MAX_PIECES <= EV_RANGE && EV_RANGE + MAX_RANGES <= EV_INDEX_FREE &&
+              EV_INDEX_FREE < EV_INDEX_READY && EV_INDEX_READY < EV_UOUT_FREE && EV_UOUT_FREE + 2 <= EV_POOL, "ev_pool slots overlap");
+
+// b200c_ctx::h_pinned: every value read back from the device lands in its own member, so no read-back overwrites a value that another
+// one still needs
+struct Pinned {
+    // codec helpers (engine.cu)
+    uint64_t packed_len;                                // pack_digest_device: compressed size of the file
+    uint32_t digest;                                    // pack_digest_device, raw_digest: Digest.crc32
+    uint64_t chunk_err;                                 // b200c_decompress_chunks / b200c_uncompress_chunks: ChunkErr
+    // OutStream (engine.cu)
+    uint64_t os_end[OutStream::MAX_PIECES];             // file offset behind packed piece s
+    uint32_t os_digest;
+    // b200c_compact (compact.cu)
+    uint64_t cerr, err;                                 // ChunkErr, DevErr
+    uint64_t range[2 * B200C_MAX_INPUTS];               // k_input_ranges: partitions [a, b) of every input
+    uint64_t scan[B200C_MAX_INPUTS + 1];                // K2: first partition of every input (and the total)
+    uint32_t bad[B200C_MAX_INPUTS + 1];                 // K2: inputs whose Summary intervals or speculation did not prove
+    uint64_t plan[2 * MAX_RANGES * B200C_MAX_INPUTS];   // k_range_plan: bytes of U every piece reads from every input
+    uint64_t nparts, class_end[4];                      // K3: output partitions, ends of the fan-in classes <= 8 / 12 / 16 / 32
+    uint64_t scratch_len, iscr_len;                     // K4: scratch bytes for Data.db and Index.db
+    uint64_t ntiles, nbig;                              // staged K4: tiles, partitions left to the thread kernels
+    uint64_t data_end, index_len, written;              // K4: end of the piece in the file, its Index.db bytes, its written partitions
+    uint64_t summary_len;                               // Summary.db entry bytes of the piece
+    uint64_t run_stats[3], hist[B200C_MAX_INPUTS], bytes_in_range;   // RunStats, merged_row_counts, bytes in the token range
+    uint64_t cut[2], file_end, file_index_len, file_stats[3];       // multi-file output: k_find_cut, end of the file, its Index.db, its RunStats
+};
+enum { H_PINNED_CAP = 1 << 16 };
+static_assert(sizeof(Pinned) <= H_PINNED_CAP, "b200c_ctx::h_pinned");
 
 // device-wide exclusive scan: out[0..n] (n+1 entries, out[n] = total). TIn = uint32_t or uint64_t. scan_slot0: first of 3 ws slots.
 template <typename TIn> int exclusive_scan(b200c_ctx* c, const TIn* in, uint64_t n, uint64_t* out, int scan_slot0, int depth = 0);

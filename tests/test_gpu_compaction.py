@@ -379,12 +379,11 @@ def test_wrong_summary_positions_only_cost_the_sequential_walk(ctx):
     assert g.data == want.data and g.index == want.index and g.digest == want.digest
     assert got.stats["index_slow_path_inputs"] == 1
 
-@pytest.mark.parametrize("env", [{"B200C_K1_BATCH": "2"}, {"B200C_K1": "0", "B200C_K1_BATCH": "0"}, {"B200C_K1": "2", "B200C_K1_BATCH": "2"}, {"B200C_K5": "3"}, {"B200C_K5": "1"},
-                                 {"B200C_K2_INTERVALS": "1"}, {"B200C_K5_OVERLAP": "1", "B200C_RANGES": "5"}])
+@pytest.mark.parametrize("env", [{"B200C_K1_BATCH": "2"}, {"B200C_K1": "0", "B200C_K1_BATCH": "0"}, {"B200C_K1": "2", "B200C_K1_BATCH": "2"}, {"B200C_K5": "3"}, {"B200C_K5": "1"}])
 def test_alternate_codec_kernels_match(env):
     """K1 mappings stay selectable for A/B (B200C_K1: 0 = warp per chunk, 1 = thread per chunk for launches of >= 32768 chunks;
     2 = two passes, lz4_batch.cuh; B200C_K1_BATCH: 1 = all inputs' chunk ranges in one launch, 2 = even for tiny launches; B200C_K5: 1 = LZ4 with
-    the hash table in shared memory, 3 = two passes, lz4_chain.cuh; B200C_K2_INTERVALS: the Index.db walk by Summary interval; B200C_K5_OVERLAP: K5 of a streamed piece on its own stream): parity must hold for all"""
+    the hash table in shared memory, 3 = two passes, lz4_chain.cuh): parity must hold for all"""
     import subprocess, sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     r = subprocess.run([sys.executable, "-m", "pytest", "-x", "-q", "-m", "gpu", "tests/test_gpu_codec.py", "tests/test_gpu_compaction.py",
