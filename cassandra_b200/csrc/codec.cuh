@@ -78,7 +78,8 @@ __global__ void __launch_bounds__(32) k_compress_chunks(const DevTables* __restr
 }
 
 // LZ4 with only the 16 KiB hash table in shared memory: the chunk is read where it lies (L1 read-only path), 13 blocks of one warp per
-// SM instead of 7. Needs a 4-byte aligned stream start and chunk length (every caller's buffers are).
+// SM instead of 7: 3 warps per scheduler, so the time is the length of one warp's chain of L2 round trips, which lz4_compress_warp<true>
+// keeps to three per sequence (lz4.cuh). Needs a 4-byte aligned stream start and chunk length (every caller's buffers are).
 template <bool DUP>
 __global__ void __launch_bounds__(32) k_compress_chunks_lz4_direct(const DevTables* __restrict__ T,
         const uint8_t* __restrict__ in, uint64_t n, int chunk_len, int max_clen,

@@ -62,9 +62,10 @@ int compress_slots_device(b200c_ctx* c, int comp, const uint8_t* d_in, uint64_t 
     uint64_t nchunks = (n + chunk_len - 1) / chunk_len;
     if (!nchunks) return B200C_OK;
     // B200C_K5: 0 = chunk copy in shared memory, 1 = the chunk read through L1, 3 = two passes (lz4_chain.cuh / snappy_chain.cuh).
-    // Unset: what measured fastest on an H100 80GB HBM3 (400 W) in bench.py's device-resident step — LZ4 mode 1 (K5 on configs[1]: 78.5 ms,
-    // mode 0: 96.3, two passes: 94.4; the link-building pass is bound by the sector traffic of its random 4-byte reads), Snappy two passes
-    // (configs[2]: 93.5 ms, mode 1: 104.3; its table is 32 KiB, 6 chunks per SM).
+    // Unset: what measured fastest on an H100 80GB HBM3 in bench.py's device-resident step — LZ4 mode 1 (K5 on configs[1] at 400 W: 78.5 ms,
+    // mode 0: 96.3, two passes: 94.4; the link-building pass is bound by the sector traffic of its random 4-byte reads; with mode 1's reads
+    // issued early, at 700 W: 60.3 ms against 78.1), Snappy two passes (configs[2]: 93.5 ms, mode 1: 104.3; its table is 32 KiB, 6 chunks per
+    // SM). Mode 2 (mode 1 with a distinct-hash scoreboard in shared memory) measured 66.1 ms against mode 1's 60.3: not the default.
     const int k5_env = []() { const char* e = getenv("B200C_K5"); return e ? atoi(e) : -1; }();
     const int k5_mode = k5_env >= 0 ? k5_env : (comp_is_snappy(comp) ? 3 : 1);
     if (k5_mode == 3 && comp == COMP_LZ4 && ((uintptr_t)d_in & 3) == 0 && (chunk_len & 3) == 0 && chunk_len <= LZ4C_MAX_CHUNK) {

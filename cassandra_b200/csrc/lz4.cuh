@@ -40,6 +40,9 @@ __device__ __forceinline__ int lz4_emit_len_ext(uint8_t* out, int rem, int lane)
 // through the read-only L1 path (ld.global.nc): only the hash table occupies shared memory then, which doubles the chunks an SM holds
 // — and this kernel is a chain of dependent instructions per chunk, so chunks in flight are what buys throughput. No byte beyond
 // position n - 1 influences the result (searches stop at n - 12, matches at n - 5), so what follows the chunk in memory is irrelevant.
+// With 13 one-warp blocks on an SM the time is the number of L2 round trips one warp waits for one after the other, so the GLOBAL path
+// issues reads as soon as their addresses are known: three dependent trips per sequence (the search window's bytes, the candidates'
+// bytes, then catch-up + literals + match length in one round) where reading each when it is used makes five. No load is past byte n - 1.
 template <bool GLOBAL> __device__ __forceinline__ uint32_t lz4_rd32(const uint32_t* in32, int p) {
     if (!GLOBAL) return rd32_at(in32, p);
     uint32_t lo = __ldg(in32 + (p >> 2)), hi = __ldg(in32 + (p >> 2) + 1);
@@ -86,6 +89,9 @@ template <bool GLOBAL> __device__ int lz4_compress_warp(const uint8_t* s_in, int
                 uint32_t seq = valid ? lz4_rd32<GLOBAL>(in32, p) : 0u;
                 uint32_t h = lz4_hash_u16(seq);
                 int cand = valid ? (int)s_tab[h] : 0;
+                // the table's candidate is nearly always the one compared: ask for its bytes before the same-hash masks are built, so that
+                // the round trip runs under the ballots; a lane whose candidate is an earlier lane of this window takes that lane's `seq`
+                uint32_t cseq = GLOBAL ? lz4_rd32<GLOBAL>(in32, cand) : 0u;
                 // lanes with the same hash. match.any costs several hundred cycles here (one pass per distinct value); 13 ballots, one
                 // per hash bit, are independent of each other and give the same mask. Invalid lanes form a suffix that neither
                 // `prev` (lower lanes only) nor the masked `later_same` tests below can reach, so they need no special key.
@@ -109,7 +115,9 @@ template <bool GLOBAL> __device__ int lz4_compress_warp(const uint8_t* s_in, int
                 int src = prev ? (31 - __clz(prev)) : lane;
                 int pc = __shfl_sync(FULL_MASK, p, src);
                 if (prev) cand = pc;
-                bool hit = valid && !putonly && (lz4_rd32<GLOBAL>(in32, cand) == seq);
+                if (GLOBAL) { const uint32_t sseq = __shfl_sync(FULL_MASK, seq, src); if (prev) cseq = sseq; }   // that lane read those four bytes
+                // (an invalid lane's `cand` may be an invalid lane's p, beyond the chunk: it must not be read)
+                bool hit = valid && !putonly && ((GLOBAL ? cseq : lz4_rd32<GLOBAL>(in32, cand)) == seq);
                 uint32_t hits = __ballot_sync(FULL_MASK, hit);
                 uint32_t inval = __ballot_sync(FULL_MASK, !valid);
                 int first_hit = hits ? (__ffs(hits) - 1) : 32;
@@ -134,31 +142,74 @@ template <bool GLOBAL> __device__ int lz4_compress_warp(const uint8_t* s_in, int
             if (ended) break;
             __syncwarp();
 
-            int lit_nibble = 0;
-            if (!immediate) {
-                // ---- catch up: extend the match backwards -----------------------------------------------------------
-                for (;;) {
-                    int j = lane + 1;
-                    bool ok = (ip - j >= anchor) && (match - j >= 0) && (lz4_rd8<GLOBAL>(s_in, ip - j) == lz4_rd8<GLOBAL>(s_in, match - j));
-                    uint32_t b = __ballot_sync(FULL_MASK, ok);
-                    int steps = (b == FULL_MASK) ? 32 : (__ffs(~b) - 1);
-                    ip -= steps; match -= steps;
-                    if (steps < 32) break;
+            int lit_nibble = 0, mc = 0;
+            if (GLOBAL) {
+                // One round of loads instead of three dependent ones. The backward extension, the first 32 literals and the first 32 bytes
+                // of the match length read at addresses that the hit alone decides: the forward compare starts at the hit's ip + 4
+                // wherever catch-up ends (the bytes between are known to be equal), and the literals start at anchor. Every chunk
+                // byte is a round trip to L2 here, so the three are asked for together and only the long cases loop.
+                const int ip0 = ip, m0 = match;
+                const bool bk = !immediate && ip0 - 1 - lane >= anchor && m0 - 1 - lane >= 0;
+                const bool fw = ip0 + LZ4_MINMATCH + lane < matchlimit;
+                const bool lt = !immediate && anchor + lane < ip0;
+                const uint32_t bi = bk ? lz4_rd8<GLOBAL>(s_in, ip0 - 1 - lane) : 0u, bm = bk ? lz4_rd8<GLOBAL>(s_in, m0 - 1 - lane) : 1u;
+                const uint32_t fi = fw ? lz4_rd8<GLOBAL>(s_in, ip0 + LZ4_MINMATCH + lane) : 0u, fm = fw ? lz4_rd8<GLOBAL>(s_in, m0 + LZ4_MINMATCH + lane) : 1u;
+                const uint32_t lb = lt ? lz4_rd8<GLOBAL>(s_in, anchor + lane) : 0u;
+                // ---- catch up ---------------------------------------------------------------------------------------
+                uint32_t b = __ballot_sync(FULL_MASK, bi == bm);
+                while (b == FULL_MASK) {
+                    ip -= 32; match -= 32;
+                    const int j = lane + 1;
+                    const bool ok = (ip - j >= anchor) && (match - j >= 0) && (lz4_rd8<GLOBAL>(s_in, ip - j) == lz4_rd8<GLOBAL>(s_in, match - j));
+                    b = __ballot_sync(FULL_MASK, ok);
                 }
+                { const int steps = __ffs(~b) - 1; ip -= steps; match -= steps; }
                 // ---- literals ---------------------------------------------------------------------------------------
-                int lit = ip - anchor;
                 token_pos = op++;
-                if (lit >= 15) op += lz4_emit_len_ext(out + op, lit - 15, lane);
-                for (int i = lane; i < lit; i += 32) out[op + i] = (uint8_t)lz4_rd8<GLOBAL>(s_in, anchor + i);
-                op += lit;
-                lit_nibble = lit < 15 ? lit : 15;
-            } else token_pos = op++;                      // immediate match: token with literal length 0
-
-            // ---- the match: offset, length beyond MINMATCH limited by matchlimit (LZ4_count) --------------------------
-            if (lane == 0) { int off = ip - match; out[op] = (uint8_t)off; out[op + 1] = (uint8_t)(off >> 8); }
-            op += 2;
-            int mc = 0;
-            {
+                if (!immediate) {
+                    const int lit = ip - anchor;
+                    if (lit >= 15) op += lz4_emit_len_ext(out + op, lit - 15, lane);
+                    if (lane < lit) out[op + lane] = (uint8_t)lb;
+                    for (int i = lane + 32; i < lit; i += 32) out[op + i] = (uint8_t)lz4_rd8<GLOBAL>(s_in, anchor + i);
+                    op += lit;
+                    lit_nibble = lit < 15 ? lit : 15;
+                }
+                // ---- the match: offset, length beyond MINMATCH limited by matchlimit (LZ4_count) ----------------------
+                if (lane == 0) { int off = ip - match; out[op] = (uint8_t)off; out[op + 1] = (uint8_t)(off >> 8); }
+                op += 2;
+                const int pi = ip0 + LZ4_MINMATCH, pm = m0 + LZ4_MINMATCH;
+                b = __ballot_sync(FULL_MASK, fi == fm);
+                int fc = 0;
+                while (b == FULL_MASK) {
+                    fc += 32;
+                    const int i = fc + lane;
+                    const bool eq = (pi + i < matchlimit) && (lz4_rd8<GLOBAL>(s_in, pi + i) == lz4_rd8<GLOBAL>(s_in, pm + i));
+                    b = __ballot_sync(FULL_MASK, eq);
+                }
+                fc += __ffs(~b) - 1;
+                mc = (ip0 - ip) + fc;                     // liblz4 counts from the caught-up ip + 4: the bytes up to the hit's ip + 4 are equal
+            } else {                                       // the chunk in shared memory: each step reads when it knows where
+                if (!immediate) {
+                    // ---- catch up: extend the match backwards -------------------------------------------------------
+                    for (;;) {
+                        int j = lane + 1;
+                        bool ok = (ip - j >= anchor) && (match - j >= 0) && (lz4_rd8<GLOBAL>(s_in, ip - j) == lz4_rd8<GLOBAL>(s_in, match - j));
+                        uint32_t b = __ballot_sync(FULL_MASK, ok);
+                        int steps = (b == FULL_MASK) ? 32 : (__ffs(~b) - 1);
+                        ip -= steps; match -= steps;
+                        if (steps < 32) break;
+                    }
+                    // ---- literals -----------------------------------------------------------------------------------
+                    int lit = ip - anchor;
+                    token_pos = op++;
+                    if (lit >= 15) op += lz4_emit_len_ext(out + op, lit - 15, lane);
+                    for (int i = lane; i < lit; i += 32) out[op + i] = (uint8_t)lz4_rd8<GLOBAL>(s_in, anchor + i);
+                    op += lit;
+                    lit_nibble = lit < 15 ? lit : 15;
+                } else token_pos = op++;                  // immediate match: token with literal length 0
+                // ---- the match: offset, length beyond MINMATCH limited by matchlimit (LZ4_count) ----------------------
+                if (lane == 0) { int off = ip - match; out[op] = (uint8_t)off; out[op + 1] = (uint8_t)(off >> 8); }
+                op += 2;
                 int pi = ip + LZ4_MINMATCH, pm = match + LZ4_MINMATCH;
                 for (;;) {
                     int i = mc + lane;
