@@ -337,8 +337,12 @@ template <class CUR> __device__ __forceinline__ int cmp_heads(const CParams& P, 
     return cmp_clust(P, a, b);
 }
 
+// header.readDeletionTime + DeletionTime.build (S/db/DeletionTime.java:54-58): an ldt below 0 (a wrapped delta) or above MAX_DELETION_TIME reads
+// as InvalidDeletionTime (ldt 2^32 - 2). Row deletions, markers and complex deletions all read through here. One unsigned compare and a select.
 __device__ __forceinline__ DT read_delta_dt(Rd& r, const InDesc& in) {
-    DT d; d.mfda = (int64_t)(r.vint() + (uint64_t)in.min_ts); d.ldt = (int64_t)r.vint32() + in.min_ldt; return d;
+    DT d; d.mfda = (int64_t)(r.vint() + (uint64_t)in.min_ts); d.ldt = (int64_t)r.vint32() + in.min_ldt;
+    d.ldt = (uint64_t)d.ldt > 0xFFFFFFFDull ? (int64_t)0xFFFFFFFEu : d.ldt;
+    return d;
 }
 __device__ __forceinline__ int64_t decode_ldt(int64_t ldt, int32_t ttl) {          // Cell.decodeLocalDeletionTime :221-239
     if (ldt >= ttl) return ldt;
@@ -346,6 +350,9 @@ __device__ __forceinline__ int64_t decode_ldt(int64_t ldt, int32_t ttl) {       
     if (ttl == 0x7FFFFFFF) return ldt;
     return (int64_t)0xFFFFFFFEu;
 }
+// the row liveness's ldt is decoded as a cell's (UnfilteredSerializer.java:596-598). Out of line: row_header is inlined into every K4 kernel, and
+// rows with a TTL are rare enough that a call costs less than the registers an inlined copy takes in the emitting kernels.
+__device__ __noinline__ int64_t decode_liveness_ldt(int64_t ldt, int32_t ttl) { return decode_ldt(ldt, ttl); }
 // DeletionTime.Serializer.deserialize (oa): S/db/DeletionTime.java:222-243
 __device__ __forceinline__ DT read_partition_dt(Rd& r) {
     uint32_t f = r.u8();
@@ -516,7 +523,7 @@ template <class CUR> __device__ __forceinline__ Rd row_header(const CParams& P, 
     Rd r{P.U, c.pos + c.body_rel, c.next, 0};
     info = live_empty(); del = dt_live();
     if (c.flags & 0x04) info.ts = (int64_t)(r.vint() + (uint64_t)in.min_ts);
-    if (c.flags & 0x08) { info.ttl = r.vint32() + in.min_ttl; info.ldt = (int64_t)r.vint32() + in.min_ldt; }
+    if (c.flags & 0x08) { info.ttl = r.vint32() + in.min_ttl; info.ldt = decode_liveness_ldt((int64_t)r.vint32() + in.min_ldt, info.ttl); }      // :596-598
     if (c.flags & 0x10) del = read_delta_dt(r, in);
     return r;
 }
@@ -634,7 +641,7 @@ __device__ __noinline__ bool cx_seek(const CParams& P, const CxVer& v, int oc, R
         PCell tmp;
         if (oci < P.cx_first) { cx_read_cell(in, r, v, P.vfix[oci], -1, &tmp); continue; }
         DT d = dt_live();
-        if (v.flags & 0x40) d = read_delta_dt(r, in);
+        if (v.flags & 0x40) { d = read_delta_dt(r, in); if (d.mfda == I64_MIN) d = dt_live(); }      // LIVE written beside another column's deletion (BTreeRow.java:770-778)
         const int32_t n = r.vint32();
         if (n < 0) { r.err = PERR_CORRUPT; return false; }
         if (oci == oc) { *cd = d; *count = (uint32_t)n; return true; }

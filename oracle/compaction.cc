@@ -192,9 +192,14 @@ static void read_clust_values(Reader& r, const Schema& s, int n, Clust& c) {
     }
 }
 
-// header.readDeletionTime: S/db/SerializationHeader.java:186-200
+// header.readDeletionTime: S/db/SerializationHeader.java:186-206, then DeletionTime.build (S/db/DeletionTime.java:54-58): a negative local
+// deletion time (the writer's (int) cast wrapped a delta of 2^31 or more) or one above Cell.MAX_DELETION_TIME reads as InvalidDeletionTime,
+// whose ldt is INVALID_DELETION_TIME. Row deletions, range tombstone markers and complex deletions all come through here; the complex
+// deletion's own "negative ldt" repair (UnfilteredSerializer.java:670-676) cannot fire on a value built this way.
 static DT read_delta_dt(Reader& r, const b200c_encoding_stats& hs) {
-    DT d; d.mfda = (int64_t)(r.vint() + (uint64_t)hs.min_timestamp); d.ldt = (int64_t)r.vint32() + hs.min_local_deletion_time; return d;
+    DT d; d.mfda = (int64_t)(r.vint() + (uint64_t)hs.min_timestamp); d.ldt = (int64_t)r.vint32() + hs.min_local_deletion_time;
+    if (d.ldt < 0 || d.ldt > (int64_t)UINT32_MAX - 2) d.ldt = (int64_t)UINT32_MAX - 1;
+    return d;
 }
 
 // DeletionTime.Serializer.deserialize (oa): S/db/DeletionTime.java:222-243
@@ -222,7 +227,9 @@ static void read_row_body(Reader& r, Source& src, uint8_t flags, int ncols_in, c
     r.vint(); r.vint();                                   // row size, previous unfiltered size
     u.info = Live(); u.del = DT();
     if (flags & 0x04) u.info.ts = (int64_t)(r.vint() + (uint64_t)hs.min_timestamp);
-    if (flags & 0x08) { u.info.ttl = r.vint32() + hs.min_ttl; u.info.ldt = (int64_t)r.vint32() + hs.min_local_deletion_time; }
+    if (flags & 0x08) {                                   // the liveness ldt is decoded as a cell's is (:596-598)
+        u.info.ttl = r.vint32() + hs.min_ttl; u.info.ldt = decode_ldt((int64_t)r.vint32() + hs.min_local_deletion_time, u.info.ttl);
+    }
     if (flags & 0x10) u.del = read_delta_dt(r, hs);
     uint64_t missing = 0;
     if (!(flags & 0x20)) {                                // Columns.deserializeSubset: S/db/Columns.java:533-560
@@ -266,7 +273,9 @@ static void read_row_body(Reader& r, Source& src, uint8_t flags, int ncols_in, c
         int64_t count = (int64_t)r.vint32();
         if (count < 0) throw Corrupt{src.idx, 4, 0, 0, "negative cell count"};
         for (int64_t k = 0; k < count; k++) read_cell(oc, t, true);
-        if (!cd.live()) u.cdel.push_back({oc, cd});
+        // BTreeRow.Builder's CellResolver (S/db/rows/BTreeRow.java:770-778) keeps a complex deletion only if its timestamp is above Long.MIN_VALUE:
+        // LIVE, written by a row that has a complex deletion in another column, reads back as (MIN_VALUE, InvalidDeletionTime) and is dropped there
+        if (cd.mfda != INT64_MIN) u.cdel.push_back({oc, cd});
     }
     std::stable_sort(u.cells.begin(), u.cells.end(), [](const CellV& a, const CellV& b) { return a.col < b.col; });
     std::sort(u.cdel.begin(), u.cdel.end(), [](const std::pair<int, DT>& a, const std::pair<int, DT>& b) { return a.first < b.first; });
