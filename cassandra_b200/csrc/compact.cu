@@ -693,8 +693,11 @@ template <bool EMIT> __device__ __forceinline__ void k4_epilogue(const K4Args& a
     a.st_munf[j] = (uint32_t)st.merged_unfiltereds; a.st_rows[j] = (uint32_t)st.rows_out;
 }
 
+// 384 threads per SM: ptxas then gives a thread 168 registers instead of 128, which takes the fan-in <= 8 emit kernel's spills from
+// 554 / 924 bytes down to 70 / 132 (they sat in the L1 that the dependent Data.db loads need). Fewer threads in flight, each one waiting
+// less: K4 on configs[1] 100.1 -> 92.1 ms on an H100 80GB HBM3 at 700 W (DESIGN §5); 640 threads at 96 registers lost
 template <int M_CAP, int NT, bool EMIT, bool CX = false>
-__global__ void __launch_bounds__(NT) k_partition_thr(const K4Args a, uint64_t lo, uint64_t hi) {
+__global__ void __launch_bounds__(NT, 384 / NT) k_partition_thr(const K4Args a, uint64_t lo, uint64_t hi) {
     extern __shared__ __align__(16) uint8_t s_raw[];
     // per thread in shared memory: M_CAP cursors, then (for tables with <= K4_SMEM_COLS columns) the merged-row scratch; +8 bytes
     // so that consecutive threads start in different banks. Wider tables keep the merged row in local memory.
