@@ -222,6 +222,104 @@ __global__ void __launch_bounds__(32) k_compress_chunks_snappy_direct(const DevT
     }
 }
 
+// ---- K5 for chunks of 128 KiB to 1 MiB ---------------------------------------------------------------------------------------------
+// A chunk this long does not fit in shared memory: it is read where it lies, as the direct kernels above read theirs. The kernels below
+// take every such chunk whatever B200C_K5 says (the switch selects among the kernels of chunks <= 64 KiB), so the output never depends on it.
+
+// the raw-storage rule and the CRC of a finished slot, as the kernels above apply them: stored raw (zero padded to max_clen) when compression
+// did not help enough, then the big-endian CRC32 of the bytes as written, the file length and the digest register
+__device__ __forceinline__ void k5_finish_slot(const DevTables* __restrict__ T, const uint8_t* src, int ulen, int clen, int max_clen, uint8_t* slot,
+                                               uint64_t chunk, uint32_t* __restrict__ file_len, uint32_t* __restrict__ seg_raw, int lane) {
+    if (clen >= max_clen) {                            // flushData :158-177
+        for (int i = lane; i < ulen; i += 32) slot[i] = src[i];
+        clen = ulen;
+        if (ulen < max_clen) { for (int i = ulen + lane; i < max_clen; i += 32) slot[i] = 0; clen = max_clen; }
+    }
+    __syncwarp();
+    __threadfence_block();
+    uint32_t raw = warp_crc32_raw(T, T->crc_adv128, slot, clen, lane);
+    uint32_t init = gf2_mulmod(0xFFFFFFFFu, warp_xpow8n(T, (uint32_t)clen, lane));
+    uint32_t crc = ~(raw ^ init);
+    if (lane == 0) {
+        slot[clen] = (uint8_t)(crc >> 24); slot[clen + 1] = (uint8_t)(crc >> 16); slot[clen + 2] = (uint8_t)(crc >> 8); slot[clen + 3] = (uint8_t)crc;
+        file_len[chunk] = (uint32_t)clen + 4;
+        uint32_t x = raw ^ __byte_perm(crc, 0, 0x0123);
+        seg_raw[chunk] = T->crc_t[3][x & 0xff] ^ T->crc_t[2][(x >> 8) & 0xff] ^ T->crc_t[1][(x >> 16) & 0xff] ^ T->crc_t[0][x >> 24];
+    }
+}
+
+// LZ4: one warp per chunk in liblz4's byU32 regime (lz4.cuh). A short last chunk below LZ4_64KLIMIT is compressed byU16, as liblz4 does.
+// Needs a 4-byte aligned stream start.
+__global__ void __launch_bounds__(32) k_compress_chunks_lz4_big(const DevTables* __restrict__ T,
+        const uint8_t* __restrict__ in, uint64_t n, int chunk_len, int max_clen,
+        uint8_t* __restrict__ slots, int slot_stride, uint32_t* __restrict__ file_len, uint32_t* __restrict__ seg_raw) {
+    __shared__ __align__(16) uint32_t s_tab[1 << LZ4_HASHLOG_U32];          // 16 KiB: 4096 x u32, or 8192 x u16 for a short last chunk
+    const int lane = threadIdx.x;
+    const uint64_t chunk = blockIdx.x;
+    const uint64_t start = chunk * (uint64_t)chunk_len;
+    const int ulen = (int)min((uint64_t)chunk_len, n - start);
+    const uint8_t* src = in + start;
+    uint8_t* slot = slots + chunk * (uint64_t)slot_stride;
+    if (lane == 0) { slot[0] = (uint8_t)ulen; slot[1] = (uint8_t)(ulen >> 8); slot[2] = (uint8_t)(ulen >> 16); slot[3] = (uint8_t)(ulen >> 24); }
+    const int clen = 4 + (ulen >= LZ4_64KLIMIT ? lz4_compress_warp<true, true>(src, ulen, s_tab, slot + 4, lane)
+                                               : lz4_compress_warp<true>(src, ulen, (uint16_t*)s_tab, slot + 4, lane));
+    k5_finish_slot(T, src, ulen, clen, max_clen, slot, chunk, file_len, seg_raw, lane);
+}
+
+// Snappy: snappy::Compress cuts its input into 64 KiB fragments (kBlockSize) and compresses each on its own with a table sized for it, so the
+// fragments of a chunk are independent. Pass 1: one warp per fragment (snappy_compress_fragment_warp) into a fragment slot; dynamic smem =
+// the table of a 64 KiB fragment. Pass 2: one warp per chunk writes the varint length and the fragments back to back, then the raw rule and CRC.
+enum { SNAPPY_BLOCK = 65536 };
+__global__ void __launch_bounds__(32) k_snappy_big_fragments(int max_bits, const uint8_t* __restrict__ in, uint64_t n, int chunk_len,
+                                                             uint8_t* __restrict__ frag_slots, int frag_stride, uint32_t* __restrict__ frag_len) {
+    extern __shared__ __align__(16) uint8_t smem_sf[];
+    uint16_t* s_tab = (uint16_t*)smem_sf;
+    const int lane = threadIdx.x;
+    const uint64_t f = blockIdx.x, fpc = (uint64_t)(chunk_len / SNAPPY_BLOCK);
+    const uint64_t start = (f / fpc) * (uint64_t)chunk_len + (f % fpc) * SNAPPY_BLOCK;
+    if (start >= n) { if (lane == 0) frag_len[f] = 0; return; }           // past the end of a short last chunk
+    const int len = (int)min((uint64_t)SNAPPY_BLOCK, n - start);
+    const int tsz = snappy_table_size(len, max_bits);
+    for (int i = lane; i < tsz / 2; i += 32) ((uint32_t*)s_tab)[i] = 0;
+    __syncwarp();
+    const int op = snappy_compress_fragment_warp<true>(in + start, 0, len, s_tab, tsz, max_bits, frag_slots + f * (uint64_t)frag_stride, 0, lane);
+    if (lane == 0) frag_len[f] = (uint32_t)op;
+}
+__global__ void __launch_bounds__(32) k_snappy_big_assemble(const DevTables* __restrict__ T, const uint8_t* __restrict__ in, uint64_t n, int chunk_len, int max_clen,
+        const uint8_t* __restrict__ frag_slots, int frag_stride, const uint32_t* __restrict__ frag_len,
+        uint8_t* __restrict__ slots, int slot_stride, uint32_t* __restrict__ file_len, uint32_t* __restrict__ seg_raw) {
+    const int lane = threadIdx.x;
+    const uint64_t chunk = blockIdx.x;
+    const uint64_t start = chunk * (uint64_t)chunk_len;
+    const int ulen = (int)min((uint64_t)chunk_len, n - start);
+    uint8_t* slot = slots + chunk * (uint64_t)slot_stride;
+    int op = 0;
+    {   uint32_t v = (uint32_t)ulen;
+        while (v >= 0x80) { if (lane == 0) slot[op] = (uint8_t)(v | 0x80); v >>= 7; op++; }
+        if (lane == 0) slot[op] = (uint8_t)v;
+        op++; }
+    const uint64_t f0 = chunk * (uint64_t)(chunk_len / SNAPPY_BLOCK);
+    for (int k = 0; k * SNAPPY_BLOCK < ulen; k++) {
+        const int len = (int)frag_len[f0 + k];
+        const uint8_t* s = frag_slots + (f0 + k) * (uint64_t)frag_stride;
+        for (int i = lane; i < len; i += 32) slot[op + i] = s[i];
+        op += len;
+    }
+    k5_finish_slot(T, in + start, ulen, op, max_clen, slot, chunk, file_len, seg_raw, lane);
+}
+
+// NoopCompressor: the chunk as it is
+__global__ void __launch_bounds__(32) k_compress_chunks_noop_big(const DevTables* __restrict__ T, const uint8_t* __restrict__ in, uint64_t n, int chunk_len, int max_clen,
+        uint8_t* __restrict__ slots, int slot_stride, uint32_t* __restrict__ file_len, uint32_t* __restrict__ seg_raw) {
+    const int lane = threadIdx.x;
+    const uint64_t chunk = blockIdx.x;
+    const uint64_t start = chunk * (uint64_t)chunk_len;
+    const int ulen = (int)min((uint64_t)chunk_len, n - start);
+    uint8_t* slot = slots + chunk * (uint64_t)slot_stride;
+    for (int i = lane; i < ulen; i += 32) slot[i] = in[start + i];
+    k5_finish_slot(T, in + start, ulen, ulen, max_clen, slot, chunk, file_len, seg_raw, lane);
+}
+
 // ---- pack: slots -> dense Data.db image --------------------------------------------------------------------------
 // one warp per chunk; offs = exclusive scan of file_len
 // out_base (optional): device scalar subtracted from the offsets, for an image buffer that holds only a window of the file
@@ -356,14 +454,11 @@ __global__ void __launch_bounds__(RAW_THREADS, 8) k_raw_checksum(const DevTables
 // stream in global memory and match sources are read back from it (a warp may read what its other lanes stored after
 // __syncwarp()). Dropping the 16 KiB staging buffer raises residency from 13 to 32 warps per SM, which is what this
 // latency-bound, strictly sequential format needs.
-__global__ void __launch_bounds__(64) k_decompress_chunks(const DevTables* __restrict__ T, int comp,
+// the warp-per-chunk decoder: chunk `chunk` of one file, lanes 0..31 of a warp
+__device__ __forceinline__ void decompress_chunk_warp(const DevTables* __restrict__ T, int comp,
         const uint8_t* __restrict__ data, uint64_t data_len, const uint64_t* __restrict__ offs, uint64_t nchunks,
         int chunk_len, int max_clen, uint64_t data_length, uint8_t* out, int verify, ChunkErr* __restrict__ err,
-        uint64_t chunk0, uint64_t chunk_end, int tag,         // this launch covers chunks [chunk0, chunk_end) of the file; tag = input number for error reports
-        const uint8_t* __restrict__ tail, uint64_t tail_off) {  // (k1_src)
-    const int lane = threadIdx.x & 31;
-    const uint64_t chunk = chunk0 + (uint64_t)blockIdx.x * 2 + (threadIdx.x >> 5);
-    if (chunk >= chunk_end || chunk >= nchunks) return;
+        uint64_t chunk, int tag, const uint8_t* __restrict__ tail, uint64_t tail_off, int lane) {
     const uint64_t off = offs[chunk];
     const uint64_t next = (chunk + 1 < nchunks) ? offs[chunk + 1] : data_len;
     const uint64_t ustart = chunk * (uint64_t)chunk_len;
@@ -395,6 +490,31 @@ __global__ void __launch_bounds__(64) k_decompress_chunks(const DevTables* __res
         if (got >= 0) for (int i = lane; i < ulen; i += 32) dst[i] = src[i];
     }
     if (got != ulen && lane == 0) report_chunk_err(err, ((uint64_t)tag << 40) | chunk, 2);
+}
+__global__ void __launch_bounds__(64) k_decompress_chunks(const DevTables* __restrict__ T, int comp,
+        const uint8_t* __restrict__ data, uint64_t data_len, const uint64_t* __restrict__ offs, uint64_t nchunks,
+        int chunk_len, int max_clen, uint64_t data_length, uint8_t* out, int verify, ChunkErr* __restrict__ err,
+        uint64_t chunk0, uint64_t chunk_end, int tag,         // this launch covers chunks [chunk0, chunk_end) of the file; tag = input number for error reports
+        const uint8_t* __restrict__ tail, uint64_t tail_off) {  // (k1_src)
+    const int lane = threadIdx.x & 31;
+    const uint64_t chunk = chunk0 + (uint64_t)blockIdx.x * 2 + (threadIdx.x >> 5);
+    if (chunk >= chunk_end || chunk >= nchunks) return;
+    decompress_chunk_warp(T, comp, data, data_len, offs, nchunks, chunk_len, max_clen, data_length, out, verify, err, chunk, tag, tail, tail_off, lane);
+}
+
+// chunks above 64 KiB of several inputs in ONE launch, one warp per chunk. Such a chunk is a long chain of dependent steps (a 1 MiB LZ4 chunk
+// holds ~10^5 sequences), so a launch lasts as long as its slowest chunk: one launch for all inputs instead of one after the other per input.
+__global__ void __launch_bounds__(64) k_decompress_multi_warp(const DevTables* __restrict__ T, const K1Seg* __restrict__ segs, int nseg, uint64_t total,
+                                                              int verify, ChunkErr* __restrict__ err) {
+    const uint64_t t = (uint64_t)blockIdx.x * 2 + (threadIdx.x >> 5);
+    if (t >= total) return;
+    int lo = 0, hi = nseg - 1;
+    while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (segs[mid].first <= t) lo = mid; else hi = mid - 1; }
+    const K1Seg& g = segs[lo];
+    const uint64_t chunk = g.chunk0 + (t - g.first);
+    if (chunk >= g.nchunks) return;
+    decompress_chunk_warp(T, g.comp, g.data, g.data_len, g.offs, g.nchunks, g.chunk_len, g.max_clen, g.data_length, g.out, verify, err, chunk, g.tag,
+                          g.tail, g.tail_off, threadIdx.x & 31);
 }
 
 // ---- K1, thread-per-chunk variant (LZ4 and stored chunks) -----------------------------------------------------------------

@@ -10,6 +10,12 @@ enum { COMP_NONE = 0, COMP_LZ4 = 1, COMP_SNAPPY = 2, COMP_SNAPPY15 = 3 };      /
 enum { COMP_UNCOMPRESSED = 4 };
 __host__ __device__ __forceinline__ bool comp_is_snappy(int c) { return c == COMP_SNAPPY || c == COMP_SNAPPY15; }
 
+// chunk lengths: powers of two up to 1 MiB (CompressionParams allows any power of two; tables raise it to 128-512 KiB for scans), up to
+// 64 KiB for CRC.db of an uncompressed table (ChecksummedSequentialWriter writes 64 KiB). Chunks above CHUNK_LEN_SMALL take their own K5 kernels.
+enum { CHUNK_LEN_SMALL = 65536, CHUNK_LEN_MAX = 1 << 20 };
+__host__ __device__ __forceinline__ bool chunk_len_supported(int comp, int chunk_len) {
+    return chunk_len > 0 && (chunk_len & (chunk_len - 1)) == 0 && chunk_len <= (comp == COMP_UNCOMPRESSED ? (int)CHUNK_LEN_SMALL : (int)CHUNK_LEN_MAX);
+}
 __host__ __device__ __forceinline__ int chunk_max_compressed(int comp, int chunk_len) {
     if (comp == COMP_LZ4) return 4 + (chunk_len + chunk_len / 255 + 16);
     if (comp_is_snappy(comp)) return (32 + chunk_len + chunk_len / 6);
@@ -28,7 +34,7 @@ __device__ __forceinline__ void report_chunk_err(ChunkErr* e, uint64_t chunk, in
 
 // one input's chunk range [chunk0, chunk0 + count) in a multi-input K1 launch; first = threads of the launch before this segment
 struct K1Seg { const uint8_t* data; uint64_t data_len; const uint64_t* offs; uint64_t nchunks; uint64_t data_length; uint8_t* out;
-               uint64_t chunk0, count, first; int chunk_len, max_clen, tag, _pad;
+               uint64_t chunk0, count, first; int chunk_len, max_clen, tag, comp;     // comp: read by k_decompress_multi_warp only (the others are LZ4)
                uint64_t rec0, rec_span;         // two-pass LZ4 (lz4_batch.cuh): first record slot of this segment, compressed bytes its slots were sized for
                const uint8_t* tail; uint64_t tail_off; };     // staged copy of the file's bytes from tail_off on (k1_src)
 

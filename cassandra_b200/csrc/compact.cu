@@ -39,6 +39,7 @@ int decompress_stream_device(b200c_ctx* c, int comp, const uint8_t* d_data, uint
                              int chunk_len, int max_clen, uint64_t data_length, uint8_t* d_out, int verify, ChunkErr* d_err, uint64_t chunk0, uint64_t count, int tag,
                              const uint8_t* tail, uint64_t tail_off);
 int decompress_multi_device(b200c_ctx* c, K1Seg* segs, int nseg, int verify, ChunkErr* d_err, int ws_slot);
+int decompress_big_device(b200c_ctx* c, K1Seg* segs, int nseg, int verify, ChunkErr* d_err, int ws_slot);
 int raw_chunks_device(b200c_ctx* c, bool ingest, const RawArgs& a);
 int raw_stream_device(b200c_ctx* c, const uint8_t* d_in, uint64_t n, int chunk_len, uint8_t* d_out, uint64_t* d_crc, uint32_t* digest, int ws_base);
 
@@ -54,7 +55,7 @@ static_assert(IW_PAD <= 64, "the Index.db workspace keeps 64 bytes behind every 
 
 enum { WS_U = 16, WS_CD, WS_CO, WS_IDX, WS_PARAMS, WS_BBASE, WS_ISTART, WS_ICNT, WS_IEND, WS_IHIT, WS_IBAD, WS_ISCAN,
        WS_TOK, WS_KP, WS_KLEN, WS_UPOS, WS_PBASE, WS_RANGE, WS_BSTART, WS_CONTRIB, WS_HEAD, WS_OPIDX, WS_OPFIRST,
-       WS_LIST, WS_CURSOR, WS_STMUNF, WS_STROWS, WS_OVF, WS_BOUND, WS_BPOS, WS_SCRATCH, WS_DSIZE, WS_IPAY, WS_NBLK, WS_IHEAD, WS_DPOS, WS_ISIZE, WS_IPOS, WS_UOUT, WS_IOUT, WS_DOUT, WS_OOFFS, WS_STATS, WS_ERR2, WS_LCS0 = 82, WS_LCS1, WS_LCS2, WS_LCS3, WS_LCS4, WS_ICAP, WS_IOFF, WS_ISCR, WS_PLAN, WS_UOUT2, WS_SUMM, WS_PURGE, WS_K1SEG, WS_INSZ, WS_BIG, WS_INPOS, WS_TMARK, WS_TSCAN, WS_TSTART, WS_META_SG, WS_META_TD, WS_META_BLOOM, WS_META_KEYS, WS_META_SUMENT, WS_META_SUMOFF, WS_META_FLAG, WS_META_WRANK, WS_META_SAMPLE, WS_META_ESIZE, WS_META_EPOS, WS_CCOUNT, WS_SLICE, WS_META_TDD, WS_K1TAIL,
+       WS_LIST, WS_CURSOR, WS_STMUNF, WS_STROWS, WS_OVF, WS_BOUND, WS_BPOS, WS_SCRATCH, WS_DSIZE, WS_IPAY, WS_NBLK, WS_IHEAD, WS_DPOS, WS_ISIZE, WS_IPOS, WS_UOUT, WS_IOUT, WS_DOUT, WS_OOFFS, WS_STATS, WS_ERR2, WS_LCS0 = 82, WS_LCS1, WS_LCS2, WS_LCS3, WS_LCS4, WS_ICAP, WS_IOFF, WS_ISCR, WS_PLAN, WS_UOUT2, WS_SUMM, WS_PURGE, WS_K1SEG, WS_INSZ, WS_BIG, WS_INPOS, WS_TMARK, WS_TSCAN, WS_TSTART, WS_META_SG, WS_META_TD, WS_META_BLOOM, WS_META_KEYS, WS_META_SUMENT, WS_META_SUMOFF, WS_META_FLAG, WS_META_WRANK, WS_META_SAMPLE, WS_META_ESIZE, WS_META_EPOS, WS_CCOUNT, WS_SLICE, WS_META_TDD, WS_K1TAIL, WS_K1SEG_BIG,
        WS_SCANA = 60, WS_CODEC = 70 };
 
 static_assert(WS_ERR2 < WS_SCANA && WS_SCANA + 6 <= WS_CODEC && WS_CODEC + 12 <= WS_LCS0 && WS_K1TAIL < WS_SLOTS, "workspace slot map");
@@ -1047,7 +1048,7 @@ struct CompactCall {
     // ---- device arrays
     uint8_t *U = nullptr, *CD = nullptr, *IDX = nullptr; uint64_t *CO = nullptr, *d_bbase = nullptr, *d_summ = nullptr; CParams* dP = nullptr;
     DevErr* d_err = nullptr; ChunkErr* d_cerr = nullptr; RunStats* d_stats = nullptr; unsigned long long *d_hist = nullptr, *d_rbytes = nullptr;
-    std::vector<const uint8_t*> k1_data, k1_tail; std::vector<const uint64_t*> k1_offs; std::vector<uint64_t> k1_tail_off; std::vector<K1Seg> segs;
+    std::vector<const uint8_t*> k1_data, k1_tail; std::vector<const uint64_t*> k1_offs; std::vector<uint64_t> k1_tail_off; std::vector<K1Seg> segs, bsegs;
     int k1_batch_env = 0;
     // metadata state (meta.cuh), device resident across the pieces of the call
     StatGlobal* d_sg = nullptr; TdropTable* d_td = nullptr; uint32_t* d_bloom = nullptr; uint8_t *d_mkeys = nullptr, *d_sument = nullptr; uint64_t* d_sumoff = nullptr;
@@ -1134,10 +1135,10 @@ struct CompactCall {
         if (m->nclustering > MAXCLUST || m->ncolumns >= 64 || m->ncolumns < 0) { c->err = "schema outside the supported envelope"; return B200C_EUNSUPPORTED; }
         for (int k = 0; k < m->nstatic_columns; k++) if ((m->static_columns[k].type >> 8) & 0xFF) { c->err = "multi-cell static column"; return B200C_EUNSUPPORTED; }
         if (res->noutputs_cap < 1 || !res->outputs) { c->err = "no output slot"; return B200C_EINVAL; }
-        if (m->out_chunk_len <= 0 || m->out_chunk_len > 65536 || (m->out_chunk_len & (m->out_chunk_len - 1))) { c->err = "output chunk_len"; return B200C_EUNSUPPORTED; }
+        if (!chunk_len_supported(m->out_compressor, m->out_chunk_len)) { c->err = "output chunk_len"; return B200C_EUNSUPPORTED; }
         for (int i = 0; i < K; i++) {
             const b200c_input& in = m->inputs[i];
-            if (in.chunk_len <= 0 || in.chunk_len > 65536 || (in.chunk_len & (in.chunk_len - 1))) { c->err = "input chunk_len"; return B200C_EUNSUPPORTED; }
+            if (!chunk_len_supported(in.compressor, in.chunk_len)) { c->err = "input chunk_len"; return B200C_EUNSUPPORTED; }
             if (in.ncolumns < 0 || in.ncolumns >= 64) { c->err = "input columns"; return B200C_EUNSUPPORTED; }
             if (in.nchunks != (in.data_length + in.chunk_len - 1) / (uint64_t)in.chunk_len) { c->err = "chunk count does not match data_length"; return B200C_EINVAL; }
             if (in.compressor != COMP_LZ4 && !comp_is_snappy(in.compressor) && in.compressor != COMP_NONE && in.compressor != COMP_UNCOMPRESSED) { c->err = "unknown compressor"; return B200C_EINVAL; }
@@ -1452,12 +1453,30 @@ struct CompactCall {
         return decompress_stream_device(c, in.compressor, k1_data[i], in.data_len, k1_offs[i], in.nchunks, in.chunk_len,
                                         in.max_compressed_len, in.data_length, U + ubase[i], 1, d_cerr, a, b - a, i, k1_tail[i], k1_tail_off[i]);
     }
-    // several inputs' chunk ranges in one thread-per-chunk launch when there are enough of them (B200C_K1_BATCH=0 switches it off)
+    // several inputs' chunk ranges in one thread-per-chunk launch when there are enough of them (B200C_K1_BATCH=0 switches it off); chunks above
+    // 64 KiB are never in it (k1_big)
+    static bool k1_batchable(const b200c_input& in) { return in.compressor == COMP_LZ4 && !(in.chunk_len & 7) && in.chunk_len <= CHUNK_LEN_SMALL; }
+    static bool big_chunks(const b200c_input& in) { return in.compressor != COMP_UNCOMPRESSED && in.chunk_len > CHUNK_LEN_SMALL; }
+    // the inputs with chunks above 64 KiB, whatever the switches say: one warp-per-chunk launch over all of them
+    int k1_big(const std::vector<uint64_t>& from, const std::vector<uint64_t>& to) {
+        bsegs.clear();
+        for (int i = 0; i < K; i++) {
+            const b200c_input& in = m->inputs[i];
+            if (from[i] >= to[i] || !big_chunks(in)) continue;
+            K1Seg g; memset(&g, 0, sizeof(g));
+            g.data = k1_data[i]; g.data_len = in.data_len; g.offs = k1_offs[i]; g.nchunks = in.nchunks; g.data_length = in.data_length; g.out = U + ubase[i];
+            g.tail = k1_tail[i]; g.tail_off = k1_tail_off[i];
+            g.chunk0 = from[i]; g.count = to[i] - from[i]; g.chunk_len = in.chunk_len; g.max_clen = in.max_compressed_len; g.tag = i; g.comp = in.compressor;
+            bsegs.push_back(g);
+        }
+        return bsegs.empty() ? B200C_OK : decompress_big_device(c, bsegs.data(), (int)bsegs.size(), 1, d_cerr, WS_K1SEG_BIG);
+    }
     int k1_many(const std::vector<uint64_t>& from, const std::vector<uint64_t>& to) {      // chunks [from[i], to[i]) of every input
+        B200C_TRY(k1_big(from, to));
         segs.clear(); uint64_t total = 0;
         for (int i = 0; i < K && k1_batch_env != 0; i++) {
             const b200c_input& in = m->inputs[i];
-            if (from[i] >= to[i] || in.compressor != COMP_LZ4 || (in.chunk_len & 7)) continue;
+            if (from[i] >= to[i] || !k1_batchable(in)) continue;
             K1Seg g; memset(&g, 0, sizeof(g));
             g.data = k1_data[i]; g.data_len = in.data_len; g.offs = k1_offs[i]; g.nchunks = in.nchunks; g.data_length = in.data_length; g.out = U + ubase[i];
             g.tail = k1_tail[i]; g.tail_off = k1_tail_off[i];
@@ -1469,7 +1488,7 @@ struct CompactCall {
         if (batched) B200C_TRY(decompress_multi_device(c, segs.data(), (int)segs.size(), 1, d_cerr, WS_K1SEG));
         for (int i = 0; i < K; i++) {
             const b200c_input& in = m->inputs[i];
-            if (batched && in.compressor == COMP_LZ4 && !(in.chunk_len & 7)) continue;
+            if (big_chunks(in) || (batched && k1_batchable(in))) continue;
             B200C_TRY(k1(i, from[i], to[i]));
         }
         return B200C_OK;
@@ -1489,12 +1508,11 @@ struct CompactCall {
         // read in place; their Index.db / Summary.db staging runs under K1 and K2 waits for it.
         if (!dev) B200C_TRY(wait_inputs());
         if (deferred) return B200C_OK;
-        if (dev && k1_batch_env != 0) {          // device-resident inputs: decode in one launch
-            std::vector<uint64_t> z(K, 0), e(K);
-            for (int i = 0; i < K; i++) e[i] = m->inputs[i].nchunks;
-            return k1_many(z, e);
-        }
-        for (int i = 0; i < K; i++) B200C_TRY(k1(i, 0, m->inputs[i].nchunks));
+        std::vector<uint64_t> z(K, 0), e(K);
+        for (int i = 0; i < K; i++) e[i] = m->inputs[i].nchunks;
+        if (dev && k1_batch_env != 0) return k1_many(z, e);          // device-resident inputs: decode in one launch
+        B200C_TRY(k1_big(z, e));
+        for (int i = 0; i < K; i++) if (!big_chunks(m->inputs[i])) B200C_TRY(k1(i, 0, m->inputs[i].nchunks));
         return B200C_OK;
     }
 

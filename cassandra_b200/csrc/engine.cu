@@ -53,6 +53,32 @@ int exclusive_scan(b200c_ctx* c, const TIn* in, uint64_t n, uint64_t* out, int s
 template int exclusive_scan<uint32_t>(b200c_ctx*, const uint32_t*, uint64_t, uint64_t*, int, int);
 template int exclusive_scan<uint64_t>(b200c_ctx*, const uint64_t*, uint64_t, uint64_t*, int, int);
 
+// K5 of chunks above 64 KiB (codec.cuh), whatever B200C_K5 says. Their kernels read the chunks in place, 4-byte aligned: a stream that starts
+// elsewhere (a file of an LCS output starts where its first partition does) is first copied to an aligned buffer.
+static int compress_big_slots_device(b200c_ctx* c, int comp, const uint8_t* d_in, uint64_t n, int chunk_len, int max_clen,
+                                     uint8_t* slots, int stride, uint32_t* file_len, uint32_t* seg_raw, uint64_t nchunks) {
+    if (((uintptr_t)d_in & 3) != 0) {
+        uint8_t* a; B200C_TRY(ws_typed(c, WS_K5_BIGIN, (size_t)n + 64, &a));
+        B200C_CUDA_TRY(c, cudaMemcpyAsync(a, d_in, n, cudaMemcpyDeviceToDevice, c->stream));
+        d_in = a;
+    }
+    if (comp == COMP_LZ4) {
+        B200C_LAUNCH(c, k_compress_chunks_lz4_big, (unsigned)nchunks, 32, 0, c->d_tables, d_in, n, chunk_len, max_clen, slots, stride, file_len, seg_raw);
+    } else if (comp_is_snappy(comp)) {
+        const int max_bits = comp == COMP_SNAPPY15 ? 15 : 14, fstride = (snappy_max_compressed_length(SNAPPY_BLOCK) + 15) & ~15;
+        const uint64_t nfrag = nchunks * (uint64_t)(chunk_len / SNAPPY_BLOCK);
+        uint8_t* frags; uint32_t* flen;
+        B200C_TRY(ws_typed(c, WS_K5_FRAGS, nfrag * (uint64_t)fstride + 64, &frags));
+        B200C_TRY(ws_typed(c, WS_K5_FLEN, nfrag + 1, &flen));
+        B200C_LAUNCH(c, k_snappy_big_fragments, (unsigned)nfrag, 32, (size_t)2 * snappy_table_size(SNAPPY_BLOCK, max_bits), max_bits, d_in, n, chunk_len, frags, fstride, flen);
+        B200C_LAUNCH(c, k_snappy_big_assemble, (unsigned)nchunks, 32, 0, c->d_tables, d_in, n, chunk_len, max_clen, (const uint8_t*)frags, fstride, (const uint32_t*)flen,
+                     slots, stride, file_len, seg_raw);
+    } else {
+        B200C_LAUNCH(c, k_compress_chunks_noop_big, (unsigned)nchunks, 32, 0, c->d_tables, d_in, n, chunk_len, max_clen, slots, stride, file_len, seg_raw);
+    }
+    return B200C_OK;
+}
+
 // device-side chunk compression of a resident stream, in two halves so that the LCS writer can compress a window, look at the
 // chunk sizes, and only then decide where the file ends:
 //   compress_slots_device: every chunk of d_in[0..n) -> its fixed-stride slot (+ CRC), file_len[i] = bytes + 4, seg_raw[i] for the digest
@@ -61,6 +87,7 @@ int compress_slots_device(b200c_ctx* c, int comp, const uint8_t* d_in, uint64_t 
                           uint8_t* slots, int stride, uint32_t* file_len, uint32_t* seg_raw) {
     uint64_t nchunks = (n + chunk_len - 1) / chunk_len;
     if (!nchunks) return B200C_OK;
+    if (chunk_len > CHUNK_LEN_SMALL) return compress_big_slots_device(c, comp, d_in, n, chunk_len, max_clen, slots, stride, file_len, seg_raw, nchunks);
     // B200C_K5: 0 = chunk copy in shared memory, 1 = the chunk read through L1, 3 = two passes (lz4_chain.cuh / snappy_chain.cuh).
     // Unset: what measured fastest on an H100 80GB HBM3 in bench.py's device-resident step — LZ4 mode 1 (K5 on configs[1] at 400 W: 78.5 ms,
     // mode 0: 96.3, two passes: 94.4; the link-building pass is bound by the sector traffic of its random 4-byte reads; with mode 1's reads
@@ -280,7 +307,8 @@ int decompress_stream_device(b200c_ctx* c, int comp, const uint8_t* d_data, uint
     static const int k1_mode = []() { const char* e = getenv("B200C_K1"); return e ? atoi(e) : 1; }();      // 0: warp per chunk, 1: thread per chunk (LZ4)
     // thread per chunk needs tens of thousands of chunks in flight to beat the warp kernel; small launches (token-range pieces of one
     // input) keep the warp mapping unless compact.cu has batched them (decompress_multi_device)
-    if (k1_mode == 1 && comp == COMP_LZ4 && (chunk_len & 7) == 0 && ((uintptr_t)d_out & 7) == 0 && end - chunk0 >= 32768)
+    // chunks above 64 KiB always take the warp kernel: one thread decoding 1 MiB is a chain 16 times longer than the L2 plan of k1_plan assumes
+    if (k1_mode == 1 && comp == COMP_LZ4 && (chunk_len & 7) == 0 && chunk_len <= CHUNK_LEN_SMALL && ((uintptr_t)d_out & 7) == 0 && end - chunk0 >= 32768)
         B200C_LAUNCH(c, k_decompress_chunks_thr, k1_grid(c, end - chunk0), K1_THREADS, c->k1_smem, c->d_tables, comp, d_data, data_len, d_offs, nchunks,
                      chunk_len, max_clen, data_length, d_out, verify, d_err, chunk0, end, tag, tail, tail_off);
     else
@@ -319,6 +347,17 @@ int decompress_multi_device(b200c_ctx* c, K1Seg* segs, int nseg, int verify, Chu
     unsigned long long* next = (unsigned long long*)(d + nseg);      // chunk counter of the launch (k_decompress_multi_thr)
     B200C_CUDA_TRY(c, cudaMemsetAsync(next, 0, sizeof(*next), c->stream));
     B200C_LAUNCH(c, k_decompress_multi_thr, k1_grid(c, total), K1_THREADS, c->k1_smem, c->d_tables, d, nseg, total, verify, d_err, next);
+    return B200C_OK;
+}
+
+// chunk ranges above 64 KiB of several inputs, any compressor, in one warp-per-chunk launch (segs: host array, first filled here)
+int decompress_big_device(b200c_ctx* c, K1Seg* segs, int nseg, int verify, ChunkErr* d_err, int ws_slot) {
+    uint64_t total = 0;
+    for (int i = 0; i < nseg; i++) { segs[i].first = total; segs[i].count = segs[i].nchunks > segs[i].chunk0 ? std::min(segs[i].count, segs[i].nchunks - segs[i].chunk0) : 0; total += segs[i].count; }
+    if (!total) return B200C_OK;
+    K1Seg* d; B200C_TRY(ws_typed(c, ws_slot, (size_t)nseg, &d));
+    B200C_CUDA_TRY(c, cudaMemcpyAsync(d, segs, sizeof(K1Seg) * nseg, cudaMemcpyHostToDevice, c->stream));
+    B200C_LAUNCH(c, k_decompress_multi_warp, (unsigned)((total + 1) / 2), 64, 0, c->d_tables, (const K1Seg*)d, nseg, total, verify, d_err);
     return B200C_OK;
 }
 
@@ -391,6 +430,7 @@ b200c_ctx* b200c_create(int device, size_t workspace_bytes) {
     if (cudaMallocHost((void**)&c->h_pinned, H_PINNED_CAP) != cudaSuccess) { cudaFree(c->d_tables); delete c; return nullptr; }
     cudaFuncSetAttribute(k_compress_chunks, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536 + 65536 + 16);
     cudaFuncSetAttribute(k_compress_chunks_snappy_direct, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536);
+    cudaFuncSetAttribute(k_snappy_big_fragments, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536);     // the 2^15 table of a 64 KiB fragment
     k1_plan(c);
     (void)workspace_bytes;
     return c;
@@ -459,7 +499,7 @@ int b200c_initial_compressed_buffer_length(int comp, int chunk_len) { return chu
 static int check_codec_args(b200c_ctx* c, int comp, int chunk_len) {
     if (!c) return B200C_EINVAL;
     if (comp != COMP_LZ4 && !comp_is_snappy(comp) && comp != COMP_NONE && comp != COMP_UNCOMPRESSED) { c->err = "unknown compressor"; return B200C_EINVAL; }
-    if (chunk_len <= 0 || chunk_len > 65536 || (chunk_len & (chunk_len - 1))) { c->err = "chunk_len must be a power of two <= 64 KiB"; return B200C_EUNSUPPORTED; }
+    if (!chunk_len_supported(comp, chunk_len)) { c->err = comp == COMP_UNCOMPRESSED ? "CRC.db chunk_len must be a power of two <= 64 KiB" : "chunk_len must be a power of two <= 1 MiB"; return B200C_EUNSUPPORTED; }
     return B200C_OK;
 }
 
@@ -585,7 +625,7 @@ int b200c_decompress_chunks(b200c_ctx* c, int comp, const uint8_t* data, uint64_
 int b200c_compress(b200c_ctx* c, int comp, const uint8_t* in, int n, uint8_t* out, int out_cap) {
     if (!c || n < 0 || !out) return B200C_EINVAL;
     if (comp == COMP_UNCOMPRESSED) { c->err = "compression disabled is not an ICompressor"; return B200C_EINVAL; }
-    if (n > 65536) { c->err = "single-buffer compress is limited to 64 KiB"; return B200C_EUNSUPPORTED; }
+    if (n > CHUNK_LEN_MAX) { c->err = "single-buffer compress is limited to 1 MiB"; return B200C_EUNSUPPORTED; }
     int chunk_len = 1; while (chunk_len < n) chunk_len <<= 1;
     if (n == 0) {   // degenerate: LZ4 of nothing = length prefix + one empty-literal token; Snappy = varint 0
         if (comp == COMP_LZ4) { if (out_cap < 5) return B200C_ETOOSMALL; memset(out, 0, 5); return 5; }
@@ -610,7 +650,7 @@ int b200c_uncompress(b200c_ctx* c, int comp, const uint8_t* in, int n, uint8_t* 
     if (comp == COMP_LZ4) { if (n < 4) { c->err = "truncated"; return B200C_ECORRUPT; } ulen = (int)((uint32_t)in[0] | ((uint32_t)in[1] << 8) | ((uint32_t)in[2] << 16) | ((uint32_t)in[3] << 24)); }
     else if (comp_is_snappy(comp)) { uint32_t v = 0; int sh = 0, i = 0; bool ok = false; for (; i < n && i < 5; i++) { v |= (uint32_t)(in[i] & 0x7f) << sh; if (!(in[i] & 0x80)) { ok = true; break; } sh += 7; } if (!ok) { c->err = "bad varint"; return B200C_ECORRUPT; } ulen = (int)v; }
     else ulen = n;
-    if (ulen < 0 || ulen > 65536) { c->err = "single-buffer uncompress is limited to 64 KiB"; return B200C_ECORRUPT; }
+    if (ulen < 0 || ulen > CHUNK_LEN_MAX) { c->err = "single-buffer uncompress is limited to 1 MiB"; return B200C_ECORRUPT; }
     if (ulen > out_cap) { c->err = "output buffer too small"; return B200C_ETOOSMALL; }
     if (ulen == 0) return 0;
     int chunk_len = 1; while (chunk_len < ulen) chunk_len <<= 1;

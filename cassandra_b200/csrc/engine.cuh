@@ -11,7 +11,9 @@
 
 namespace b200c {
 
-enum { WS_SLOTS = 160, WS_K5_ENT = 150, WS_K1_REC = 151, WS_K1_NSEQ = 152 };      // (slots 0..15: codec calls, 16..: compact.cu's map, 150: K5's hash-chain entries, 151-152: K1's sequence records)
+enum { WS_SLOTS = 160, WS_K5_ENT = 150, WS_K1_REC = 151, WS_K1_NSEQ = 152, WS_K5_BIGIN = 153, WS_K5_FRAGS = 154, WS_K5_FLEN = 155 };
+// (slots 0..15: codec calls, 16..: compact.cu's map, 150: K5's hash-chain entries, 151-152: K1's sequence records, 153-155: K5 of chunks above
+//  64 KiB: an aligned copy of a misaligned stream, Snappy's fragment slots and lengths)
 
 struct WsBuf { void* p = nullptr; size_t cap = 0; };
 

@@ -1,5 +1,6 @@
-// lz4.cuh — warp-cooperative LZ4 block codec for sm_90a, bit-exact with liblz4's LZ4_compress_default for inputs
-// below 64 KiB + 11 (the 16-bit-index hash table regime every SSTable chunk length <= 64 KiB falls in).
+// lz4.cuh — warp-cooperative LZ4 block codec for sm_90a, bit-exact with liblz4's LZ4_compress_default: below 64 KiB + 11 bytes in the
+// 16-bit-index hash table regime every SSTable chunk length <= 64 KiB falls in (byU16), above it in the 32-bit-index regime of chunks of
+// 128 KiB to 1 MiB (byU32: 4096 entries hashed from 5 bytes, candidates farther back than 65535 bytes are not matches).
 //
 // Replaces the JNI boundary of S/io/compress/LZ4Compressor.java:113-134 (compress) and :136-190 (uncompress).
 // One warp owns one chunk. The greedy match finder is sequential by definition (the hash table state after position i
@@ -13,10 +14,17 @@
 namespace b200c {
 
 enum { LZ4_MINMATCH = 4, LZ4_MFLIMIT = 12, LZ4_LASTLITERALS = 5, LZ4_MINLENGTH = 13, LZ4_HASHLOG_U16 = 13,
-       LZ4_TABLE_ENTRIES = 1 << LZ4_HASHLOG_U16, LZ4_64KLIMIT = 65536 + 11 };
+       LZ4_TABLE_ENTRIES = 1 << LZ4_HASHLOG_U16, LZ4_64KLIMIT = 65536 + 11, LZ4_HASHLOG_U32 = 12, LZ4_DISTANCE_MAX = 65535 };
 
 __host__ __device__ __forceinline__ int lz4_compress_bound(int n) { return n + n / 255 + 16; }
 __device__ __forceinline__ uint32_t lz4_hash_u16(uint32_t seq) { return (seq * 2654435761u) >> (32 - LZ4_HASHLOG_U16); }
+// LZ4_hash5 of a 64-bit build: the 5 bytes at the position (seq = the first four, b4 = the fifth) times prime5bytes, top 12 bits
+__device__ __forceinline__ uint32_t lz4_hash_u32(uint32_t seq, uint32_t b4) {
+    return (uint32_t)((((((uint64_t)b4 << 32) | seq) << 24) * 889523592379ull) >> (64 - LZ4_HASHLOG_U32));
+}
+// the table entry type of a regime: byU16 for inputs below LZ4_64KLIMIT, byU32 from there on (LZ4_compress_fast_extState)
+template <bool U32> struct Lz4Tab { typedef uint16_t T; };
+template <> struct Lz4Tab<true> { typedef uint32_t T; };
 
 // distance from the search start of attempt a: steps are 1 for the first 64 attempts after the initial one, then grow by one
 // every 64 attempts (LZ4_skipTrigger = 6, acceleration = 1)
@@ -52,8 +60,13 @@ template <bool GLOBAL> __device__ __forceinline__ uint32_t lz4_rd8(const uint8_t
 
 // s_dup (optional, LZ4_DUP_ENTRIES bytes of shared memory, any content): lets a search window prove in five instructions that no two of its
 // attempts share a hash — the usual case — instead of building the same-hash masks with 13 ballots.
+// U32 (needs GLOBAL, n >= LZ4_64KLIMIT): liblz4's byU32 regime — s_tab is 4096 x u32 (16 KiB as well), the hash reads a fifth byte (the
+// high word the GLOBAL read fetched anyway) and a candidate more than LZ4_DISTANCE_MAX bytes back is no match (its slot is still updated).
 enum { LZ4_DUP_ENTRIES = 2048 };
-template <bool GLOBAL> __device__ int lz4_compress_warp(const uint8_t* s_in, int n, uint16_t* s_tab, uint8_t* out, int lane, uint8_t* s_dup = nullptr) {
+template <bool GLOBAL, bool U32 = false> __device__ int lz4_compress_warp(const uint8_t* s_in, int n, typename Lz4Tab<U32>::T* s_tab, uint8_t* out, int lane,
+                                                                         uint8_t* s_dup = nullptr) {
+    static_assert(GLOBAL || !U32, "the byU32 regime reads the chunk in place");
+    constexpr int HASHLOG = U32 ? LZ4_HASHLOG_U32 : LZ4_HASHLOG_U16;
     const uint32_t* in32 = (const uint32_t*)s_in;
     {   // zero the hash table: 16 KiB, 16 bytes per lane per step
         uint4* t4 = (uint4*)s_tab;
@@ -86,8 +99,15 @@ template <bool GLOBAL> __device__ int lz4_compress_warp(const uint8_t* s_in, int
                     int pn = fwd + lz4_attempt_offset(a + 1);
                     valid = pn <= mfl1;
                 }
-                uint32_t seq = valid ? lz4_rd32<GLOBAL>(in32, p) : 0u;
-                uint32_t h = lz4_hash_u16(seq);
+                uint32_t seq, h;
+                if constexpr (U32) {
+                    const uint32_t lo = valid ? __ldg(in32 + (p >> 2)) : 0u, hi = valid ? __ldg(in32 + (p >> 2) + 1) : 0u, sh = (p & 3) * 8;
+                    seq = __funnelshift_r(lo, hi, sh);
+                    h = lz4_hash_u32(seq, (hi >> sh) & 0xffu);
+                } else {
+                    seq = valid ? lz4_rd32<GLOBAL>(in32, p) : 0u;
+                    h = lz4_hash_u16(seq);
+                }
                 int cand = valid ? (int)s_tab[h] : 0;
                 // the table's candidate is nearly always the one compared: ask for its bytes before the same-hash masks are built, so that
                 // the round trip runs under the ballots; a lane whose candidate is an earlier lane of this window takes that lane's `seq`
@@ -109,7 +129,7 @@ template <bool GLOBAL> __device__ int lz4_compress_warp(const uint8_t* s_in, int
                 if (unique) same = 1u << lane;
                 else {
 #pragma unroll
-                    for (int b = 0; b < LZ4_HASHLOG_U16; b++) { uint32_t mb = __ballot_sync(FULL_MASK, (h >> b) & 1u); same &= ((h >> b) & 1u) ? mb : ~mb; }
+                    for (int b = 0; b < HASHLOG; b++) { uint32_t mb = __ballot_sync(FULL_MASK, (h >> b) & 1u); same &= ((h >> b) & 1u) ? mb : ~mb; }
                 }
                 uint32_t prev = same & lt_mask;
                 int src = prev ? (31 - __clz(prev)) : lane;
@@ -118,6 +138,7 @@ template <bool GLOBAL> __device__ int lz4_compress_warp(const uint8_t* s_in, int
                 if (GLOBAL) { const uint32_t sseq = __shfl_sync(FULL_MASK, seq, src); if (prev) cseq = sseq; }   // that lane read those four bytes
                 // (an invalid lane's `cand` may be an invalid lane's p, beyond the chunk: it must not be read)
                 bool hit = valid && !putonly && ((GLOBAL ? cseq : lz4_rd32<GLOBAL>(in32, cand)) == seq);
+                if constexpr (U32) hit = hit && p - cand <= LZ4_DISTANCE_MAX;
                 uint32_t hits = __ballot_sync(FULL_MASK, hit);
                 uint32_t inval = __ballot_sync(FULL_MASK, !valid);
                 int first_hit = hits ? (__ffs(hits) - 1) : 32;
@@ -125,7 +146,7 @@ template <bool GLOBAL> __device__ int lz4_compress_warp(const uint8_t* s_in, int
                 if (first_hit < first_inv) {
                     uint32_t le = (first_hit == 31) ? FULL_MASK : ((2u << first_hit) - 1u);
                     uint32_t later_same = same & le & ~lt_mask & ~(1u << lane);
-                    if (lane <= first_hit && !later_same) s_tab[h] = (uint16_t)p;
+                    if (lane <= first_hit && !later_same) s_tab[h] = (typename Lz4Tab<U32>::T)p;
                     ip = __shfl_sync(FULL_MASK, p, first_hit);
                     match = __shfl_sync(FULL_MASK, cand, first_hit);
                     immediate = prefixed && first_hit == 1;
@@ -134,7 +155,7 @@ template <bool GLOBAL> __device__ int lz4_compress_warp(const uint8_t* s_in, int
                 if (first_inv < 32) { ended = true; break; }
                 {
                     uint32_t later_same = same & ~lt_mask & ~(1u << lane);
-                    if (!later_same) s_tab[h] = (uint16_t)p;
+                    if (!later_same) s_tab[h] = (typename Lz4Tab<U32>::T)p;
                 }
                 __syncwarp();
                 a0 += prefixed ? 30 : 32;

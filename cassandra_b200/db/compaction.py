@@ -13,7 +13,7 @@ import ctypes as C, time
 import numpy as np
 from .. import native
 from ..io import sstable as sst
-from ..io.compress import CompressionMetadata, ChecksumMetadata, COMPRESSOR_IDS, COMPRESSOR_NAMES
+from ..io.compress import CompressionMetadata, ChecksumMetadata, COMPRESSOR_IDS, COMPRESSOR_NAMES, check_chunk_length
 
 INT64_MIN, INT64_MAX = -(1 << 63), (1 << 63) - 1
 
@@ -94,6 +94,7 @@ class CompactionTask:
             for name, t in i.static_columns: sunion[name] = t
         out_static = sorted(sunion.items(), key=lambda kv: _name_key(kv[0]))
         if len(out_static) > native.MAX_STATIC_COLUMNS: raise native.UnsupportedError(native.EUNSUPPORTED, "more than %d static columns" % native.MAX_STATIC_COLUMNS)
+        for c in [i.compression for i in ins] + [self.compression]: check_chunk_length(c.chunk_length, isinstance(c, ChecksumMetadata))
         m = native.Manifest(); m.abi_version = native.ABI_VERSION; m.ninputs = len(ins)
         arr = (native.Input * len(ins))(); self._keep.append(arr)
         for k, s in enumerate(ins):

@@ -58,6 +58,15 @@ class NoopCompressor(ICompressor):
     @classmethod
     def create(cls, ctx, options=None): return cls(ctx)
 
+MAX_CHUNK_LENGTH = 1 << 20                  # chunk_length_in_kb up to 1024 (include/b200c.h: B200C_MAX_CHUNK_LEN)
+MAX_CRC_CHUNK_LENGTH = 65536               # CRC.db of an uncompressed table (ChecksummedSequentialWriter writes 64 KiB)
+
+def check_chunk_length(chunk_length, uncompressed=False):
+    """CompressionParams accepts any power of two; the engine compacts chunks up to 1 MiB (CRC.db chunks up to 64 KiB) and refuses the rest."""
+    limit = MAX_CRC_CHUNK_LENGTH if uncompressed else MAX_CHUNK_LENGTH
+    if chunk_length <= 0 or chunk_length & (chunk_length - 1) or chunk_length > limit:
+        raise native.UnsupportedError(native.EUNSUPPORTED, "chunk length %d: a power of two <= %d is supported" % (chunk_length, limit))
+
 COMPRESSOR_IDS = {"LZ4Compressor": native.COMP_LZ4, "SnappyCompressor": native.COMP_SNAPPY, "NoopCompressor": native.COMP_NONE}
 COMPRESSOR_NAMES = {v: k for k, v in COMPRESSOR_IDS.items()}
 
@@ -97,6 +106,7 @@ class CompressionMetadata:
 def write_compressed(ctx, compressor: ICompressor, stream: bytes, chunk_length=16384, max_compressed_length=native.INT32_MAX):
     """CompressedSequentialWriter over a whole uncompressed stream (S/io/compress/CompressedSequentialWriter.java:140-206):
     -> (Data.db bytes, CompressionInfo.db bytes, Digest.crc32 text)."""
+    check_chunk_length(chunk_length)
     image, offs, digest = ctx.compress_chunks(compressor.compressor_id, stream, chunk_length, max_compressed_length)
     meta = CompressionMetadata(compressor.simple_name, chunk_length, max_compressed_length, len(stream), offs)
     return image, meta.serialize(), str(digest)

@@ -115,6 +115,10 @@ uint64_t     b200c_total_kernel_launches(b200c_ctx*);
 int          b200c_last_stage_ms(b200c_ctx*, double* out, int n);
 
 /* ---- chunk codec: the CompressedSequentialWriter / CompressedChunkReader data plane, batched ---------------------
+ * chunk_len (here and in b200c_input / b200c_manifest): a power of two <= B200C_MAX_CHUNK_LEN (chunk_length_in_kb up to 1024), <= 64 KiB
+ * for B200C_COMP_UNCOMPRESSED (CRC.db); anything else is B200C_EUNSUPPORTED. LZ4 chunks of at least 65547 bytes are compressed in liblz4's
+ * byU32 regime (LZ4_compress_default on an input that long), shorter ones byU16; Snappy chunks above 64 KiB are snappy::Compress's
+ * concatenation of independently compressed 64 KiB fragments behind one varint length.
  * b200c_compress_chunks: `in[0..n)` is an uncompressed Data stream. Chunk i = bytes [i*chunk_len, min((i+1)*chunk_len, n)).
  * Writes the Data.db image to `out`: for every chunk the compressor output (LZ4: 4-byte LE length + block) followed by the
  * 4-byte big-endian CRC32 of the bytes as written; chunk_offsets[i] = file offset of chunk i (CompressionInfo.db payload);
@@ -125,6 +129,7 @@ int          b200c_last_stage_ms(b200c_ctx*, double* out, int n);
  * every caller-owned device buffer must be 16-byte aligned and keep >= B200C_DEVICE_SLACK readable (for outputs: writable) bytes
  * behind its last used byte. b200c_dev_alloc adds that slack itself; plain cudaMalloc'ed buffers must be sized accordingly. */
 #define B200C_DEVICE_SLACK 256
+#define B200C_MAX_CHUNK_LEN (1 << 20)
 uint64_t     b200c_compress_bound(int compressor, uint64_t n, int chunk_len);
 uint64_t     b200c_chunk_count(uint64_t n, int chunk_len);
 int          b200c_compress_chunks(b200c_ctx*, int compressor, const uint8_t* in, uint64_t n, int chunk_len,
@@ -138,8 +143,8 @@ int          b200c_decompress_chunks(b200c_ctx*, int compressor, const uint8_t* 
                                      uint64_t data_length, uint8_t* out, int verify_crc, b200c_corruption* where, int flags);
 #define B200C_FLAG_DEVICE_PTRS 1
 
-/* ICompressor single-buffer contract (degenerate one-chunk batch; PCIe-latency bound — the batched calls are the fast path).
- * Return the number of bytes written to `out`, or a negative error code. */
+/* ICompressor single-buffer contract (degenerate one-chunk batch; PCIe-latency bound — the batched calls are the fast path): buffers of up to
+ * B200C_MAX_CHUNK_LEN uncompressed bytes. Return the number of bytes written to `out`, or a negative error code. */
 int          b200c_initial_compressed_buffer_length(int compressor, int chunk_len);
 int          b200c_compress(b200c_ctx*, int compressor, const uint8_t* in, int n, uint8_t* out, int out_cap);
 int          b200c_uncompress(b200c_ctx*, int compressor, const uint8_t* in, int n, uint8_t* out, int out_cap);

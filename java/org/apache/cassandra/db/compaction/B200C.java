@@ -27,6 +27,7 @@ public final class B200C
     public static final int MAX_COMPLEX_COLUMNS = 8;       // multi-cell (map / set / list) columns per table, B200C_MAX_COMPLEX_COLUMNS
     public static final int ABI_VERSION = 2;
     public static final int MAX_CLUSTERING = 8, MAX_COLUMNS = 64, MAX_INPUTS = 64, MAX_STATIC_COLUMNS = 16;
+    public static final int MAX_CHUNK_LENGTH = 1 << 20;      // compression chunk_length_in_kb up to 1024 (CRC.db chunks of uncompressed tables: 64 KiB)
 
     // ---- lifecycle ----------------------------------------------------------------------------------------------------------
     public static native int    abiVersion();                                       // b200c_abi_version

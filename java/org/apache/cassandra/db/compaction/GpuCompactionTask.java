@@ -91,6 +91,7 @@ public class GpuCompactionTask extends CompactionTask
             if (clusteringClass(c.type) < 0) return false;
         if (cfs.getCompactionStrategyManager().getCompactionParams().tombstoneOption() != org.apache.cassandra.schema.CompactionParams.TombstoneOption.NONE) return false;
         if (t.enforceStrictLiveness()) return false;
+        if (t.params.compression.isEnabled() && t.params.compression.chunkLength() > B200C.MAX_CHUNK_LENGTH) return false;   // (the output's chunks)
         for (SSTableReader r : inputs)
         {
             if (!(r instanceof BigTableReader) || !r.descriptor.version.version.equals("oa")) return false;
@@ -102,7 +103,7 @@ public class GpuCompactionTask extends CompactionTask
                 continue;
             }
             String comp = r.getCompressionMetadata().parameters.getSstableCompressor().getClass().getSimpleName();
-            if (compressorId(comp) < 0 || r.getCompressionMetadata().chunkLength() > 65536) return false;
+            if (compressorId(comp) < 0 || r.getCompressionMetadata().chunkLength() > B200C.MAX_CHUNK_LENGTH) return false;
         }
         return B200C.deviceCount() > 0;
     }
